@@ -39,7 +39,7 @@
 extern "C" {
 #endif
 
-#define SB_ABI_VERSION 1
+#define SB_ABI_VERSION 2
 
 /* status codes */
 #define SB_OK            0
@@ -178,6 +178,30 @@ int sb_find_batch_device(const sb_stream* image, const sb_stream* tmpl, int64_t 
 int sb_match_curves(const sb_stream* image, const sb_stream* tmpl, int64_t count,
                     const int64_t* tmpl_off, const int64_t* tmpl_len,
                     const int64_t* lag0, const int64_t* nlags, float* curves_out);
+/* ---- many streams in one call (ABI version 2) ------------------------------
+ *
+ * The same queries as sb_find_batch / sb_match_curves, but every query names its own image and template stream:
+ * query q matches streams[tmpl_slot[q]][tmpl_off[q] .. +tmpl_len[q]) against streams[image_slot[q]] over positions
+ * [lag0[q], lag0[q]+nlags[q]).  A value depends only on (template, absolute position), so queries of different
+ * streams -- different episodes of a season -- share one launch without changing any result: each result equals what
+ * sb_find_batch / sb_match_curves return for that query alone, bit for bit.  Per-query rules are theirs, checked
+ * against the query's own streams.  All streams must share one sample type and carry running sums; a NULL entry,
+ * a slot outside [0, n_streams), a stream without running sums or mixed sample types fail with SB_EINVAL, and
+ * sb_last_error() names the query or slot.
+ * The packed engine (2, 4, 5 at the default geometry) runs the whole call in one set of launches whatever the number
+ * of streams; queries of the blocked class (templates of 12+ partitions) and other engines / geometries run as one
+ * sb_find_batch-like pass per distinct (image, template) pair inside the call. */
+int sb_find_multi(const sb_stream* const* streams, int32_t n_streams, int64_t count,
+                  const int32_t* image_slot, const int32_t* tmpl_slot,
+                  const int64_t* tmpl_off, const int64_t* tmpl_len,
+                  const int64_t* lag0, const int64_t* nlags,
+                  float* diff_out, int64_t* idx_out);
+/* Whole curves of the queries above, concatenated in query order into curves_out[sum(nlags)] (host). */
+int sb_match_curves_multi(const sb_stream* const* streams, int32_t n_streams, int64_t count,
+                          const int32_t* image_slot, const int32_t* tmpl_slot,
+                          const int64_t* tmpl_off, const int64_t* tmpl_len,
+                          const int64_t* lag0, const int64_t* nlags, float* curves_out);
+
 /* The whole curve of one query (debug / parity tests): curve_out[nlags]. */
 int sb_match_curve(const sb_stream* image, const sb_stream* tmpl,
                    int64_t tmpl_off, int64_t tmpl_len, int64_t lag0, int64_t nlags,

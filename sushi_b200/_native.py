@@ -14,12 +14,13 @@ LIB_PATH = os.path.join(_HERE, 'libsushi_b200.so')
 
 SB_OK = 0
 SB_U8, SB_F32 = 0, 1
-ABI_VERSION = 1
+ABI_VERSION = 2
 
 c_i64 = ctypes.c_int64
 c_i64p = ctypes.POINTER(ctypes.c_int64)
 c_f32p = ctypes.POINTER(ctypes.c_float)
 c_vp = ctypes.c_void_p
+c_i32p = ctypes.POINTER(ctypes.c_int32)
 
 # name -> (restype, argtypes); the test-suite checks this table against the header.
 PROTOTYPES = {
@@ -57,6 +58,10 @@ PROTOTYPES = {
     'sb_find_batch': (ctypes.c_int, [c_vp, c_vp, c_i64, c_i64p, c_i64p, c_i64p, c_i64p, c_f32p, c_i64p]),
     'sb_find_batch_device': (ctypes.c_int, [c_vp, c_vp, c_i64, c_i64p, c_i64p, c_i64p, c_i64p, c_vp, c_vp]),
     'sb_match_curves': (ctypes.c_int, [c_vp, c_vp, c_i64, c_i64p, c_i64p, c_i64p, c_i64p, c_f32p]),
+    'sb_find_multi': (ctypes.c_int, [ctypes.POINTER(c_vp), ctypes.c_int32, c_i64, c_i32p, c_i32p, c_i64p, c_i64p, c_i64p, c_i64p,
+                                     c_f32p, c_i64p]),
+    'sb_match_curves_multi': (ctypes.c_int, [ctypes.POINTER(c_vp), ctypes.c_int32, c_i64, c_i32p, c_i32p, c_i64p, c_i64p, c_i64p,
+                                             c_i64p, c_f32p]),
     'sb_match_curve': (ctypes.c_int, [c_vp, c_vp, c_i64, c_i64, c_i64, c_i64, c_f32p]),
     'sb_load_pcm': (ctypes.c_int, [c_vp, c_i64, ctypes.c_int, ctypes.c_int, ctypes.c_int, ctypes.c_int,
                                    c_i64, c_i64, ctypes.POINTER(c_vp)]),

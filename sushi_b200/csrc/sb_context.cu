@@ -180,7 +180,7 @@ int sb_shutdown(void) {
     pool_release_all();
     fused_release_tables();
     packed_release_tables();
-    cudaFree(c.d_parts); cudaFree(c.d_items); cudaFree(c.d_desc); cudaFree(c.d_keys); cudaFree(c.d_groups);
+    cudaFree(c.d_parts); cudaFree(c.d_items); cudaFree(c.d_desc); cudaFree(c.d_keys); cudaFree(c.d_groups); cudaFree(c.d_multi);
     cudaFree(c.d_diff); cudaFree(c.d_idx);
     cudaFreeHost(c.h_desc); cudaFreeHost(c.h_diff); cudaFreeHost(c.h_idx);
     for (auto e : c.event_pool) cudaEventDestroy(e);

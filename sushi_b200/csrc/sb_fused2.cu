@@ -830,8 +830,20 @@ __device__ __forceinline__ void finish_item_v3(const Item& it, int tid, const Sm
     after_read();
 }
 
+// Multi-stream calls: the streams of query q (processing order) from the call's stream table -- image slot .x, template
+// slot .y -- in place of the kernel's stream arguments.
+template <typename S> struct QueryStreams { const float4* Xhat; int64_t nblk; const S* img; int64_t img_n; const double2* ipfx; const double2* tpfx; };
+template <typename S>
+__device__ __forceinline__ QueryStreams<S> select_streams(const StreamEntry* streams, const int2* slots, int q) {
+    const int2 sl = slots[q];
+    const StreamEntry si = streams[sl.x];
+    return {reinterpret_cast<const float4*>(si.specq), si.nblk, static_cast<const S*>(si.raw), si.n, si.pfx, streams[sl.y].pfx};
+}
+#define SB_SELECT_STREAMS(q) do { const QueryStreams<S> qs__ = select_streams<S>(streams, slots, (q)); \
+    Xhat = qs__.Xhat; nblk = qs__.nblk; img = qs__.img; img_n = qs__.img_n; ipfx = qs__.ipfx; tpfx = qs__.tpfx; } while (0)
+
 // ---------------------------------------------------------------- kernel A: one CTA per item
-template <typename S, int EPI>
+template <typename S, int EPI, bool MULTI = false>
 __global__ void __launch_bounds__(QT, 1)
 k_match_packed(const float4* __restrict__ That, int64_t part_first,
                const float4* __restrict__ Xhat, int64_t nblk,
@@ -839,7 +851,8 @@ k_match_packed(const float4* __restrict__ That, int64_t part_first,
                const double2* __restrict__ ipfx, const double2* __restrict__ tpfx,
                const QueryDesc* __restrict__ desc, const int* __restrict__ item_query, int64_t item_first,
                PackedTables tab, unsigned long long* __restrict__ keys, float* __restrict__ curve_out,
-               RunRecord* __restrict__ recs, int* __restrict__ rec_count) {
+               RunRecord* __restrict__ recs, int* __restrict__ rec_count,
+               const StreamEntry* __restrict__ streams = nullptr, const int2* __restrict__ slots = nullptr) {
     constexpr int T = QT, NW = QNW;
     constexpr bool is_u8 = sizeof(S) == 1;
     extern __shared__ __align__(16) unsigned char smem_raw[];
@@ -856,6 +869,7 @@ k_match_packed(const float4* __restrict__ That, int64_t part_first,
     const int tid = threadIdx.x, lane = tid & 31, warp = tid >> 5;
     const Item it(desc, item_query, item_first, blockIdx.x);
     const QueryDesc& d = it.d;
+    if constexpr (MULTI) SB_SELECT_STREAMS(it.q);
 
     // ---------------- 0. stage what the epilogue needs; the latency hides behind the MAC and the FFT
     if (is_u8) {
@@ -955,7 +969,7 @@ __device__ __forceinline__ void unpark(const float4* pk, const Buf& buf, int col
 // (the FFT buffer and the epilogue's arrays take 170-188 KB of the 227 KB), so it is parked in global memory:
 // one 128 KB slot per resident CTA (park_acquire), written and read with L2-only accesses, which L2 keeps
 // (132 slots = 17 MB of the 50 MB).  Every thread reads back exactly what it wrote, so the park needs no barrier.
-template <typename S, int EPI>
+template <typename S, int EPI, bool MULTI = false>
 __global__ void __launch_bounds__(QT, 1)
 k_match_pair(const float4* __restrict__ That, int64_t part_first,
              const float4* __restrict__ Xhat, int64_t nblk,
@@ -964,7 +978,8 @@ k_match_pair(const float4* __restrict__ That, int64_t part_first,
              const QueryDesc* __restrict__ desc, const int* __restrict__ pair_query, int64_t pair_first, int64_t n_pairs,
              float4* __restrict__ park, int* __restrict__ park_busy, int park_slots,
              PackedTables tab, unsigned long long* __restrict__ keys, float* __restrict__ curve_out,
-             RunRecord* __restrict__ recs, int* __restrict__ rec_count) {
+             RunRecord* __restrict__ recs, int* __restrict__ rec_count,
+             const StreamEntry* __restrict__ streams = nullptr, const int2* __restrict__ slots = nullptr) {
     constexpr int T = QT, NW = QNW;
     constexpr bool is_u8 = sizeof(S) == 1;
     extern __shared__ __align__(16) unsigned char smem_raw[];
@@ -1003,6 +1018,8 @@ k_match_pair(const float4* __restrict__ That, int64_t part_first,
     const bool first = !kPrefetch || pi == (int64_t)blockIdx.x;
     const int q = first ? __ldg(pair_query + pi) : *s_next_q;
     const QueryDesc d = first ? desc[q] : *s_next_d;
+    // a CTA's walk crosses query boundaries, and with them stream boundaries: every pair reads its query's entries
+    if constexpr (MULTI) SB_SELECT_STREAMS(q);
     const int64_t pi_next = pi + gridDim.x;
     int q_next = 0;
     if (kPrefetch && tid == 32 && pi_next < n_pairs) q_next = __ldg(pair_query + pi_next);      // used after the multiply phase: no wait here
@@ -1123,11 +1140,12 @@ k_match_pair(const float4* __restrict__ That, int64_t part_first,
 // EPI 3, second step: one thread per record slot evaluates the 8 lags of its run exactly (fp64) and merges the best
 // into the query's key -- the arithmetic of finish_item's exact path, with the window sums taken from the running
 // sums (for uint8 streams the same exact integers the match kernel slides on its staged bytes).
-template <typename S>
+template <typename S, bool MULTI = false>
 __global__ void __launch_bounds__(128)
 k_finish_runs(const RunRecord* __restrict__ recs, const int* __restrict__ rec_count, int64_t n_ctas,
               const QueryDesc* __restrict__ desc, const double2* __restrict__ ipfx, int64_t img_n,
-              const double2* __restrict__ tpfx, unsigned long long* __restrict__ keys) {
+              const double2* __restrict__ tpfx, unsigned long long* __restrict__ keys,
+              const StreamEntry* __restrict__ streams = nullptr, const int2* __restrict__ slots = nullptr) {
     const int64_t idx = (int64_t)blockIdx.x * blockDim.x + threadIdx.x;
     const int64_t cta = idx / kRunSlots;
     const int slot = (int)(idx - cta * kRunSlots);
@@ -1138,6 +1156,10 @@ k_finish_runs(const RunRecord* __restrict__ recs, const int* __restrict__ rec_co
     const float cc[8] = {c0.x, c0.y, c0.z, c0.w, c1.x, c1.y, c1.z, c1.w};
     const int q = head.x;
     const int64_t j0 = (int64_t)(unsigned)head.z | ((int64_t)head.w << 32);
+    if constexpr (MULTI) {
+        const int2 sl = slots[q];
+        ipfx = streams[sl.x].pfx; img_n = streams[sl.x].n; tpfx = streams[sl.y].pfx;
+    }
     const QueryDesc d = desc[q];
     const int64_t n = d.tlen, jlo = d.lag0, jhi = d.lag0 + d.nlags;
     const double2 t_hi = tpfx[d.toff + n], t_lo = tpfx[d.toff];
@@ -1171,11 +1193,15 @@ __global__ void k_fill_pair_query(const QueryDesc* __restrict__ desc, int q_begi
 // Same transform as k_forward_rows in sb_fused.cu (gather + centring + 2B-point real FFT through the
 // shared-memory inverse passes run backwards); only the output stage differs: bins leave as the chunks
 // A[i] = (X[i], X[i+B/2]) and M[i] = (X[B-i], X[B/2-i]) the packed kernel multiplies.
-template <typename S, int MODE>
+// MULTI: MODE 0 builds the rows row_list[blockIdx.x] = (slot, row) of several streams, each into its own stream's
+// rows; MODE 1 reads every query's template from its template slot.
+template <typename S, int MODE, bool MULTI = false>
 __global__ void __launch_bounds__(Cfg<14>::T, 1)
 k_forward_quad(const S* __restrict__ src, int64_t src_n, const double2* __restrict__ pfx,
                const QueryDesc* __restrict__ desc, int q_begin, int q_end, int64_t row_first,
-               FusedTables tab, float4* __restrict__ out) {
+               FusedTables tab, float4* __restrict__ out,
+               const StreamEntry* __restrict__ streams = nullptr, const int2* __restrict__ slots = nullptr,
+               const int2* __restrict__ row_list = nullptr) {
     typedef Cfg<14> C;
     constexpr int N = C::N, T = C::T, B = C::N;
     constexpr int NT2 = C::R2 * 32, NT3 = C::R3 * 32;
@@ -1191,7 +1217,14 @@ k_forward_quad(const S* __restrict__ src, int64_t src_n, const double2* __restri
 
     int64_t off, len;          // samples [off, off+len) of src, zero beyond
     float centre;
-    const int64_t row = row_first + blockIdx.x;
+    int64_t row = row_first + blockIdx.x, out_row = blockIdx.x;
+    if constexpr (MULTI && MODE == 0) {
+        const int2 rl = row_list[blockIdx.x];
+        const StreamEntry se = streams[rl.x];
+        src = static_cast<const S*>(se.raw); src_n = se.n; pfx = se.pfx;
+        out = reinterpret_cast<float4*>(se.specq);
+        row = out_row = rl.y;
+    }
     if (MODE == 0) {
         off = row * B;
         len = src_n - off; if (len > 2 * B) len = 2 * B; if (len < 0) len = 0;
@@ -1204,6 +1237,7 @@ k_forward_quad(const S* __restrict__ src, int64_t src_n, const double2* __restri
         }
         __syncthreads();
         const QueryDesc d = desc[s_q];
+        if constexpr (MULTI) { src = static_cast<const S*>(streams[slots[s_q].y].raw); pfx = streams[slots[s_q].y].pfx; }
         const int64_t seg0 = (row - d.partBase) * B;
         off = d.toff + seg0;
         len = d.tlen - seg0; if (len > B) len = B;
@@ -1232,7 +1266,7 @@ k_forward_quad(const S* __restrict__ src, int64_t src_n, const double2* __restri
         xk = make_float2(xe.x + tv.x, xe.y + tv.y);
         xbk = make_float2(xe.x - tv.x, -(xe.y - tv.y));
     };
-    float4* o = out + (int64_t)blockIdx.x * QROW;
+    float4* o = out + out_row * QROW;
     for (int i = tid; i <= Q4; i += T) {
         float2 x_i, x_bi, x_h, x_hb;
         bins(i, x_i, x_bi);                          // X[i], X[B-i]
@@ -1313,21 +1347,22 @@ __global__ void k_fill_item_query2(const QueryDesc* __restrict__ desc, int q_beg
 int* g_item_query2 = nullptr;
 int64_t g_item_query2_cap = 0;
 
-template <typename S, int MODE>
+template <typename S, int MODE, bool MULTI = false>
 int launch_forward_quad_typed(const sb_stream* src, const QueryDesc* d_desc, int q_begin, int q_end,
-                              int64_t row_first, int64_t rows, float2* out) {
+                              int64_t row_first, int64_t rows, float2* out, const MultiArgs* m = nullptr,
+                              const int2* row_list = nullptr) {
     Ctx& c = ctx();
     FusedTables tab;
     SB_TRY(fused_tables(14, &tab));
     static bool attr_set = false;
     const size_t smem = forward_smem_bytes14();
     if (!attr_set) {
-        SB_CUDA(cudaFuncSetAttribute(k_forward_quad<S, MODE>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem));
+        SB_CUDA(cudaFuncSetAttribute(k_forward_quad<S, MODE, MULTI>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem));
         attr_set = true;
     }
-    k_forward_quad<S, MODE><<<(unsigned)rows, Cfg<14>::T, smem, c.stream>>>(
+    k_forward_quad<S, MODE, MULTI><<<(unsigned)rows, Cfg<14>::T, smem, c.stream>>>(
         static_cast<const S*>(src->d_raw), src->n, src->d_pfx, d_desc, q_begin, q_end, row_first, tab,
-        reinterpret_cast<float4*>(out));
+        reinterpret_cast<float4*>(out), MULTI ? m->d_streams : nullptr, MULTI ? m->d_slots : nullptr, row_list);
     SB_CUDA(cudaGetLastError());
     return SB_OK;
 }
@@ -1379,12 +1414,17 @@ int ensure_park() {
     return SB_OK;
 }
 
-template <typename S>
-int launch_finish_runs(const sb_stream* image, const sb_stream* tmpl, const QueryDesc* d_desc, int64_t n_ctas, unsigned long long* d_keys) {
+// Stand-in for the image / template arguments of a multi-stream launch (the kernels read the table instead)
+const sb_stream kNoStream{};
+
+template <typename S, bool MULTI>
+int launch_finish_runs(const sb_stream* image, const sb_stream* tmpl, const QueryDesc* d_desc, int64_t n_ctas, unsigned long long* d_keys,
+                       const MultiArgs* m) {
     Ctx& c = ctx();
     const int64_t threads = n_ctas * kRunSlots;
-    k_finish_runs<S><<<(unsigned)((threads + 127) / 128), 128, 0, c.stream>>>(g_run_recs, g_run_count, n_ctas, d_desc, image->d_pfx, image->n,
-                                                                            tmpl->d_pfx, d_keys);
+    k_finish_runs<S, MULTI><<<(unsigned)((threads + 127) / 128), 128, 0, c.stream>>>(g_run_recs, g_run_count, n_ctas, d_desc, image->d_pfx, image->n,
+                                                                                   tmpl->d_pfx, d_keys, MULTI ? m->d_streams : nullptr,
+                                                                                   MULTI ? m->d_slots : nullptr);
     c.launches += 1;
     SB_CUDA(cudaGetLastError());
     return SB_OK;
@@ -1393,15 +1433,15 @@ int launch_finish_runs(const sb_stream* image, const sb_stream* tmpl, const Quer
 // Launchers of the three match kernels.  `Kernel` is one instantiation (sample type x epilogue variant); its
 // dynamic shared memory limit is raised once.  The uint8 kernels exist with both epilogues (Ctx::epilogue),
 // float32 streams have the first one only.
-template <typename S, int EPI>
+template <typename S, int EPI, bool MULTI>
 int launch_packed_typed(const sb_stream* image, const sb_stream* tmpl, const float2* d_parts, int64_t part_first,
                         const QueryDesc* d_desc, int64_t item_first, int64_t n_items, const PackedTables& tab,
-                        unsigned long long* d_keys, float* d_curve) {
+                        unsigned long long* d_keys, float* d_curve, const MultiArgs* m) {
     Ctx& c = ctx();
     static bool attr_set = false;
     const size_t smem = packed_smem_bytes(EPI);
     if (!attr_set) {
-        SB_CUDA(cudaFuncSetAttribute(k_match_packed<S, EPI>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem));
+        SB_CUDA(cudaFuncSetAttribute(k_match_packed<S, EPI, MULTI>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem));
         attr_set = true;
     }
     const bool records = EPI == 3 && d_curve == nullptr;             // the debug curve evaluates every lag in the kernel
@@ -1409,25 +1449,26 @@ int launch_packed_typed(const sb_stream* image, const sb_stream* tmpl, const flo
     for (int64_t i0 = 0; i0 < n_items; i0 += max_grid) {
         const int64_t ni = std::min<int64_t>(max_grid, n_items - i0);
         if (records) SB_TRY(ensure_run_records(ni));
-        k_match_packed<S, EPI><<<(unsigned)ni, QT, smem, c.stream>>>(
+        k_match_packed<S, EPI, MULTI><<<(unsigned)ni, QT, smem, c.stream>>>(
             reinterpret_cast<const float4*>(d_parts), part_first, reinterpret_cast<const float4*>(image->d_specq), image->nblkq,
             static_cast<const S*>(image->d_raw), image->n, image->d_pfx, tmpl->d_pfx, d_desc, g_item_query2 + i0, item_first + i0,
-            tab, d_keys, d_curve, records ? g_run_recs : nullptr, records ? g_run_count : nullptr);
-        if (records) SB_TRY(launch_finish_runs<S>(image, tmpl, d_desc, ni, d_keys));
+            tab, d_keys, d_curve, records ? g_run_recs : nullptr, records ? g_run_count : nullptr,
+            MULTI ? m->d_streams : nullptr, MULTI ? m->d_slots : nullptr);
+        if (records) SB_TRY((launch_finish_runs<S, MULTI>(image, tmpl, d_desc, ni, d_keys, m)));
     }
     SB_CUDA(cudaGetLastError());
     return SB_OK;
 }
 
-template <typename S, int EPI>
+template <typename S, int EPI, bool MULTI>
 int launch_pair_typed(const sb_stream* image, const sb_stream* tmpl, const float2* d_parts, int64_t part_first,
                       const QueryDesc* d_desc, int64_t pair_first, int64_t n_pairs, const PackedTables& tab,
-                      unsigned long long* d_keys, float* d_curve) {
+                      unsigned long long* d_keys, float* d_curve, const MultiArgs* m) {
     Ctx& c = ctx();
     static bool attr_set = false;
     const size_t smem = packed_smem_bytes(EPI) + 16;
     if (!attr_set) {
-        SB_CUDA(cudaFuncSetAttribute(k_match_pair<S, EPI>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem));
+        SB_CUDA(cudaFuncSetAttribute(k_match_pair<S, EPI, MULTI>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem));
         attr_set = true;
     }
     const bool records = EPI == 3 && d_curve == nullptr;             // the debug curve evaluates every lag in the kernel
@@ -1436,20 +1477,24 @@ int launch_pair_typed(const sb_stream* image, const sb_stream* tmpl, const float
         const int64_t ni = std::min<int64_t>(max_grid, n_pairs - i0);
         if (records) SB_TRY(ensure_run_records(ni));
         const int64_t grid = EPI == 3 ? std::min<int64_t>(ni, c.sm_count) : ni;      // body 3 is persistent: one CTA per SM walks the pairs
-        k_match_pair<S, EPI><<<(unsigned)grid, QT, smem, c.stream>>>(
+        k_match_pair<S, EPI, MULTI><<<(unsigned)grid, QT, smem, c.stream>>>(
             reinterpret_cast<const float4*>(d_parts), part_first, reinterpret_cast<const float4*>(image->d_specq), image->nblkq,
             static_cast<const S*>(image->d_raw), image->n, image->d_pfx, tmpl->d_pfx, d_desc, g_item_query2 + i0, pair_first + i0, ni,
-            g_park, g_park_busy, g_park_slots, tab, d_keys, d_curve, records ? g_run_recs : nullptr, records ? g_run_count : nullptr);
+            g_park, g_park_busy, g_park_slots, tab, d_keys, d_curve, records ? g_run_recs : nullptr, records ? g_run_count : nullptr,
+            MULTI ? m->d_streams : nullptr, MULTI ? m->d_slots : nullptr);
         SB_CUDA(cudaGetLastError());
-        if (records) SB_TRY(launch_finish_runs<S>(image, tmpl, d_desc, ni, d_keys));
+        if (records) SB_TRY((launch_finish_runs<S, MULTI>(image, tmpl, d_desc, ni, d_keys, m)));
     }
     return SB_OK;
 }
 
-// One instantiation per (sample type, epilogue): float32 streams have the first screening loop only.
-#define SB_DISPATCH_MATCH(FN, image, ...) \
-    ((image)->dtype != SB_U8 ? FN<float, 1>(image, __VA_ARGS__) \
-     : ctx().epilogue == 3   ? FN<uint8_t, 3>(image, __VA_ARGS__) : FN<uint8_t, 1>(image, __VA_ARGS__))
+// One instantiation per (sample type, epilogue, multi-stream): float32 streams have the first screening loop only.
+#define SB_DISPATCH_MATCH1(FN, M, dtype, ...) \
+    ((dtype) != SB_U8        ? FN<float, 1, M>(__VA_ARGS__) \
+     : ctx().epilogue == 3   ? FN<uint8_t, 3, M>(__VA_ARGS__) : FN<uint8_t, 1, M>(__VA_ARGS__))
+#define SB_DISPATCH_MATCH(FN, image, tmpl, multi, ...) \
+    ((multi) ? SB_DISPATCH_MATCH1(FN, true, (multi)->dtype, &kNoStream, &kNoStream, __VA_ARGS__, multi) \
+             : SB_DISPATCH_MATCH1(FN, false, (image)->dtype, image, tmpl, __VA_ARGS__, multi))
 
 }  // namespace
 
@@ -1459,19 +1504,19 @@ bool packed_supports(int B) { return B == QB; }
 
 int launch_match_packed(const sb_stream* image, const sb_stream* tmpl, const float2* d_parts, int64_t part_first,
                         const QueryDesc* d_desc, int q_begin, int q_end, int64_t item_first, int64_t n_items,
-                        unsigned long long* d_keys, float* d_curve) {
+                        unsigned long long* d_keys, float* d_curve, const MultiArgs* multi) {
     Ctx& c = ctx();
     PackedTables tab;
     SB_TRY(ensure_packed_tables(&tab));
     SB_TRY(ensure_item_query(n_items));
     k_fill_item_query2<<<(unsigned)(q_end - q_begin), 128, 0, c.stream>>>(d_desc, q_begin, item_first, g_item_query2);
     c.launches += 1;
-    return SB_DISPATCH_MATCH(launch_packed_typed, image, tmpl, d_parts, part_first, d_desc, item_first, n_items, tab, d_keys, d_curve);
+    return SB_DISPATCH_MATCH(launch_packed_typed, image, tmpl, multi, d_parts, part_first, d_desc, item_first, n_items, tab, d_keys, d_curve);
 }
 
 int launch_match_pair(const sb_stream* image, const sb_stream* tmpl, const float2* d_parts, int64_t part_first,
                       const QueryDesc* d_desc, int q_begin, int q_end, int64_t pair_first, int64_t n_pairs,
-                      unsigned long long* d_keys, float* d_curve) {
+                      unsigned long long* d_keys, float* d_curve, const MultiArgs* multi) {
     Ctx& c = ctx();
     PackedTables tab;
     SB_TRY(ensure_packed_tables(&tab));
@@ -1479,7 +1524,7 @@ int launch_match_pair(const sb_stream* image, const sb_stream* tmpl, const float
     SB_TRY(ensure_park());
     k_fill_pair_query<<<(unsigned)(q_end - q_begin), 128, 0, c.stream>>>(d_desc, q_begin, pair_first, g_item_query2, 2);
     c.launches += 1;
-    return SB_DISPATCH_MATCH(launch_pair_typed, image, tmpl, d_parts, part_first, d_desc, pair_first, n_pairs, tab, d_keys, d_curve);
+    return SB_DISPATCH_MATCH(launch_pair_typed, image, tmpl, multi, d_parts, part_first, d_desc, pair_first, n_pairs, tab, d_keys, d_curve);
 }
 
 int launch_block_spectra_quad(const sb_stream* s, int64_t k_first, int64_t rows, float2* out) {
@@ -1487,8 +1532,16 @@ int launch_block_spectra_quad(const sb_stream* s, int64_t k_first, int64_t rows,
                              : launch_forward_quad_typed<float, 0>(s, nullptr, 0, 0, k_first, rows, out);
 }
 
+int launch_block_spectra_quad_multi(const MultiArgs& m, const int2* d_row_list, int64_t n_rows) {
+    return m.dtype == SB_U8 ? launch_forward_quad_typed<uint8_t, 0, true>(&kNoStream, nullptr, 0, 0, 0, n_rows, nullptr, &m, d_row_list)
+                            : launch_forward_quad_typed<float, 0, true>(&kNoStream, nullptr, 0, 0, 0, n_rows, nullptr, &m, d_row_list);
+}
+
 int launch_part_spectra_quad(const sb_stream* tmpl, const QueryDesc* d_desc, int q_begin, int q_end,
-                             int64_t part_first, int64_t rows, float2* out) {
+                             int64_t part_first, int64_t rows, float2* out, const MultiArgs* multi) {
+    if (multi)
+        return multi->dtype == SB_U8 ? launch_forward_quad_typed<uint8_t, 1, true>(&kNoStream, d_desc, q_begin, q_end, part_first, rows, out, multi)
+                                     : launch_forward_quad_typed<float, 1, true>(&kNoStream, d_desc, q_begin, q_end, part_first, rows, out, multi);
     return tmpl->dtype == SB_U8 ? launch_forward_quad_typed<uint8_t, 1>(tmpl, d_desc, q_begin, q_end, part_first, rows, out)
                                 : launch_forward_quad_typed<float, 1>(tmpl, d_desc, q_begin, q_end, part_first, rows, out);
 }

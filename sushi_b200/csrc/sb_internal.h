@@ -69,6 +69,7 @@ struct Ctx {
     QueryDesc* d_desc = nullptr; int64_t desc_cap = 0;
     int2* d_groups = nullptr; int64_t groups_cap = 0;      // (query, first local lag block) per multiply group
     unsigned long long* d_keys = nullptr; int64_t keys_cap = 0;
+    unsigned char* d_multi = nullptr; int64_t multi_cap = 0;   // multi-stream calls: stream table, per-query slots, spectrum row list
     float* d_diff = nullptr; int64_t* d_idx = nullptr; int64_t res_cap = 0;
     // pinned staging
     QueryDesc* h_desc = nullptr; int64_t h_desc_cap = 0;
@@ -106,16 +107,32 @@ void pool_release_all();
 
 // engine 2 (sb_fused2.cu): spectrum rows in the quad layout, kQuadRowF2 float2 per row (128-byte aligned)
 constexpr int kQuadRowF2 = 16400;
+
+// One stream of a multi-stream call (sb_find_multi / sb_match_curves_multi), as the packed kernels read it: its
+// quad-layout spectrum rows and their count, its raw samples and their count, its running sums.  The table is built
+// per call and uploaded next to the descriptors; a second array gives every query (processing order) its image slot
+// (.x) and template slot (.y).  All streams of one call share a sample type.
+struct StreamEntry {
+    float2* specq; int64_t nblk;
+    const void* raw; int64_t n;
+    const double2* pfx;
+};
+struct MultiArgs { const StreamEntry* d_streams; const int2* d_slots; int dtype; };
+
 bool packed_supports(int B);
+// multi == nullptr: one image and one template stream (the kernels compiled as before); otherwise image / tmpl are
+// ignored and every query reads its streams from the table
 int launch_match_packed(const sb_stream* image, const sb_stream* tmpl, const float2* d_parts, int64_t part_first,
                         const QueryDesc* d_desc, int q_begin, int q_end, int64_t item_first, int64_t n_items,
-                        unsigned long long* d_keys, float* d_curve);
+                        unsigned long long* d_keys, float* d_curve, const MultiArgs* multi = nullptr);
 int launch_match_pair(const sb_stream* image, const sb_stream* tmpl, const float2* d_parts, int64_t part_first,
                       const QueryDesc* d_desc, int q_begin, int q_end, int64_t pair_first, int64_t n_pairs,
-                      unsigned long long* d_keys, float* d_curve);
+                      unsigned long long* d_keys, float* d_curve, const MultiArgs* multi = nullptr);
 int launch_block_spectra_quad(const sb_stream* s, int64_t k_first, int64_t rows, float2* out);
+// block spectra rows of several streams in one launch: row_list[i] = (slot, row)
+int launch_block_spectra_quad_multi(const MultiArgs& multi, const int2* d_row_list, int64_t n_rows);
 int launch_part_spectra_quad(const sb_stream* tmpl, const QueryDesc* d_desc, int q_begin, int q_end,
-                             int64_t part_first, int64_t rows, float2* out);
+                             int64_t part_first, int64_t rows, float2* out, const MultiArgs* multi = nullptr);
 void packed_release_tables();
 
 bool fused_supports(int B);

@@ -16,6 +16,8 @@
 #include <cmath>
 #include <cstdlib>
 #include <cstring>
+#include <map>
+#include <vector>
 
 namespace sb { int ensure_spectra(sb_stream* s, int hd); int ensure_spectra_quad(sb_stream* s, int64_t k_lo, int64_t k_hi); }
 using namespace sb;
@@ -367,12 +369,40 @@ int grow(T** p, int64_t* cap, int64_t need, bool pinned = false) {
 // been re-measured on the H100.
 constexpr int64_t kBlockedFromPartitions = 12;
 
+// The streams of one call.  The single-stream entry points pass {image, tmpl} and no slots; a multi-stream call
+// (sb_find_multi) passes its stream table and per-query image / template slots.
+struct StreamSet {
+    const sb_stream* image1 = nullptr; const sb_stream* tmpl1 = nullptr;                  // single-stream calls
+    const sb_stream* const* s = nullptr; int64_t n = 0;                                     // multi-stream calls
+    const int32_t* islot = nullptr; const int32_t* tslot = nullptr;
+    const sb_stream* image(int64_t q) const { return islot ? s[islot[q]] : image1; }
+    const sb_stream* tmpl(int64_t q) const { return tslot ? s[tslot[q]] : tmpl1; }
+    bool multi() const { return islot != nullptr; }
+};
+StreamSet pair_of(const sb_stream* image, const sb_stream* tmpl) { StreamSet ss; ss.image1 = image; ss.tmpl1 = tmpl; return ss; }
+
+// The per-query rules of every matcher entry point (q names the query in the caller's arrays)
+int check_query(const sb_stream* image, const sb_stream* tmpl, int64_t q, int64_t o, int64_t n, int64_t s, int64_t L) {
+    if (n < 1 || L < 1) SB_FAIL(SB_EINVAL, "query %lld: template length %lld / lag count %lld must be >= 1", (long long)q, (long long)n, (long long)L);
+    if (o < 0 || o + n > tmpl->n) SB_FAIL(SB_EINVAL, "query %lld: template [%lld,+%lld) outside template stream of %lld samples", (long long)q, (long long)o, (long long)n, (long long)tmpl->n);
+    if (s < 0 || s + L - 1 + n > image->n) SB_FAIL(SB_EINVAL, "query %lld: search span [%lld,+%lld)+%lld outside image stream of %lld samples", (long long)q, (long long)s, (long long)L, (long long)n, (long long)image->n);
+    if (L > 0xffffffffll) SB_FAIL(SB_EINVAL, "query %lld: more than 2^32 lags", (long long)q);
+    return SB_OK;
+}
+
+// Whether a template of n samples takes the register-blocked multiply route (engines 1-5 at hop H = B / hd)
+bool blocked_class(int64_t n, int64_t H) {
+    const Ctx& c = ctx();
+    if (c.premac_mode == 1) return false;
+    return c.premac_mode == 2 || (n + H - 1) / H >= kBlockedFromPartitions;
+}
+
 // Validate + plan a batch on the host.  Fills c.h_desc[0..count) in PROCESSING order: first the queries
 // whose multiply runs inside the fused kernel, then (from *n_direct on) those routed through the
 // register-blocked multiply kernel.  The route depends only on the query itself (its partition count),
 // never on what else is in the batch, so a given (template, position) always takes the same arithmetic
 // path.  QueryDesc::orig maps back to the caller's order; curve offsets follow the caller's order.
-int plan_batch(const sb_stream* image, const sb_stream* tmpl, int64_t count,
+int plan_batch(const StreamSet& ss, int64_t count,
                const int64_t* toff, const int64_t* tlen, const int64_t* lag0, const int64_t* nlags,
                int hd, bool allow_blocked, int direct_group, int64_t* n_direct_out,
                int64_t* total_items, int64_t* total_parts, int64_t* total_groups, int64_t* max_query_parts) {
@@ -385,18 +415,11 @@ int plan_batch(const sb_stream* image, const sb_stream* tmpl, int64_t count,
         SB_CUDA(cudaMallocHost((void**)&c.h_desc, sizeof(QueryDesc) * std::max<int64_t>(count, 64)));
         c.h_desc_cap = std::max<int64_t>(count, 64);
     }
-    auto blocked = [&](int64_t n) {
-        if (!allow_blocked || c.premac_mode == 1) return false;
-        return c.premac_mode == 2 || (n + H - 1) / H >= kBlockedFromPartitions;
-    };
+    auto blocked = [&](int64_t n) { return allow_blocked && blocked_class(n, H); };
     int64_t n_direct = 0;
     for (int64_t q = 0; q < count; ++q) {
-        const int64_t n = tlen[q], L = nlags[q], o = toff[q], s = lag0[q];
-        if (n < 1 || L < 1) SB_FAIL(SB_EINVAL, "query %lld: template length %lld / lag count %lld must be >= 1", (long long)q, (long long)n, (long long)L);
-        if (o < 0 || o + n > tmpl->n) SB_FAIL(SB_EINVAL, "query %lld: template [%lld,+%lld) outside template stream of %lld samples", (long long)q, (long long)o, (long long)n, (long long)tmpl->n);
-        if (s < 0 || s + L - 1 + n > image->n) SB_FAIL(SB_EINVAL, "query %lld: search span [%lld,+%lld)+%lld outside image stream of %lld samples", (long long)q, (long long)s, (long long)L, (long long)n, (long long)image->n);
-        if (L > 0xffffffffll) SB_FAIL(SB_EINVAL, "query %lld: more than 2^32 lags", (long long)q);
-        if (!blocked(n)) ++n_direct;
+        SB_TRY(check_query(ss.image(q), ss.tmpl(q), q, toff[q], tlen[q], lag0[q], nlags[q]));
+        if (!blocked(tlen[q])) ++n_direct;
     }
     int64_t items = 0, parts = 0, maxp = 0, groups = 0;
     int64_t pos_direct = 0, pos_blocked = n_direct;
@@ -424,13 +447,49 @@ int plan_batch(const sb_stream* image, const sb_stream* tmpl, int64_t count,
     return SB_OK;
 }
 
+// Rows of the block spectra the queries of a multi-stream call read and that are not built yet, as (slot, row) pairs:
+// run_batch builds them for every image stream in ONE launch of the forward kernel.  The bookkeeping per stream is
+// ensure_spectra_quad's: the built range [specq_lo, specq_hi) stays contiguous and is extended on either side.
+int spectra_rows_multi(const StreamSet& ss, int64_t count, StreamEntry* table, std::vector<int2>& rows) {
+    Ctx& c = ctx();
+    std::vector<int64_t> lo(ss.n, INT64_MAX), hi(ss.n, 0);
+    for (int64_t q = 0; q < count; ++q) {
+        const QueryDesc& d = c.h_desc[q];
+        const int32_t i = ss.islot[d.orig];
+        lo[i] = std::min<int64_t>(lo[i], d.k0);
+        hi[i] = std::max<int64_t>(hi[i], (int64_t)d.k0 + d.nk + d.P);
+    }
+    for (int64_t i = 0; i < ss.n; ++i) {
+        if (lo[i] == INT64_MAX) continue;
+        sb_stream* s = const_cast<sb_stream*>(ss.s[i]);
+        const int64_t nblk = (s->n + c.B - 1) / c.B;
+        const int64_t k_lo = std::max<int64_t>(lo[i], 0), k_hi = std::min<int64_t>(hi[i], nblk);
+        if (k_lo >= k_hi) continue;
+        if (!s->d_specq) {
+            SB_TRY(pool_alloc((void**)&s->d_specq, sizeof(float2) * (size_t)nblk * kQuadRowF2));
+            s->nblkq = nblk; s->specq_lo = s->specq_hi = k_lo;
+        }
+        auto add = [&](int64_t a, int64_t b) { for (int64_t k = a; k < b; ++k) rows.push_back(make_int2((int)i, (int)k)); };
+        if (s->specq_lo == s->specq_hi) { add(k_lo, k_hi); s->specq_lo = k_lo; s->specq_hi = k_hi; }
+        else {
+            if (k_lo < s->specq_lo) { add(k_lo, s->specq_lo); s->specq_lo = k_lo; }
+            if (k_hi > s->specq_hi) { add(s->specq_hi, k_hi); s->specq_hi = k_hi; }
+        }
+        table[i].specq = s->d_specq; table[i].nblk = s->nblkq;
+    }
+    return SB_OK;
+}
+
 // Core: descriptors on host (validated here), results to device arrays d_diff/d_idx.
-int run_batch(const sb_stream* image_c, const sb_stream* tmpl, int64_t count,
+// Multi-stream calls (ss.multi()) run the packed engine's direct class only (sb_find_multi routes everything else
+// through single-stream calls); every kernel then reads its query's streams from a table uploaded here.
+int run_batch(const StreamSet& ss, int64_t count,
               const int64_t* toff, const int64_t* tlen, const int64_t* lag0, const int64_t* nlags,
               float* d_diff, int64_t* d_idx, float* d_curve) {
     Ctx& c = ctx();
-    sb_stream* image = const_cast<sb_stream*>(image_c);
-    if (image->dtype != tmpl->dtype) SB_FAIL(SB_EINVAL, "image and template streams differ in sample type");
+    sb_stream* image = const_cast<sb_stream*>(ss.image(0));
+    const sb_stream* tmpl = ss.tmpl(0);
+    if (!ss.multi() && image->dtype != tmpl->dtype) SB_FAIL(SB_EINVAL, "image and template streams differ in sample type");
     if (count > 0x7fffffffll) SB_FAIL(SB_EINVAL, "more than 2^31 queries in one batch");
     const int B = c.B;
     const bool use_fused = c.engine >= 1 && fused_supports(B);
@@ -456,8 +515,9 @@ int run_batch(const sb_stream* image_c, const sb_stream* tmpl, int64_t count,
     const bool use_packed = c.engine >= 2 && packed_supports(B) && hd == 1;
     const int nb = B + 1;                                    // float2 per classic spectrum row
     int64_t n_direct = 0, total_items = 0, total_parts = 0, total_groups = 0, maxp = 0;
-    SB_TRY(plan_batch(image, tmpl, count, toff, tlen, lag0, nlags, hd, use_fused && hd == 1, 2, &n_direct,
+    SB_TRY(plan_batch(ss, count, toff, tlen, lag0, nlags, hd, use_fused && hd == 1, 2, &n_direct,
                       &total_items, &total_parts, &total_groups, &maxp));
+    if (ss.multi() && (!use_packed || n_direct != count)) SB_FAIL(SB_EINVAL, "internal: a multi-stream batch must be packed direct-class only");
     // Packed kernels: one CTA per lag block, or one per pair of consecutive lag blocks of a query (shared template
     // rows, 2P+1 row reads instead of 4P, second product spectrum parked in L2).  Both give bit-identical results;
     // pairs pay from about four partitions per template (H100 SXM at 400 W, 1000 queries at +-120 s on 30-min streams:
@@ -469,7 +529,33 @@ int run_batch(const sb_stream* image_c, const sb_stream* tmpl, int64_t count,
         for (int64_t q = 0; q < n_direct; ++q) { rows += (double)c.h_desc[q].nk * c.h_desc[q].P; blocks += (double)c.h_desc[q].nk; }
         use_pairs = rows >= 4.0 * blocks;
     }
-    if (use_packed && n_direct > 0) {
+    // multi-stream calls: the stream table (StreamEntry per slot), the slots of every query in processing order and
+    // the row list of the block spectra, in one device buffer
+    MultiArgs multi{};
+    const MultiArgs* mp = nullptr;
+    if (ss.multi()) {
+        const size_t tb = (sizeof(StreamEntry) * ss.n + 15) & ~(size_t)15, sb = (sizeof(int2) * count + 15) & ~(size_t)15;
+        int64_t max_rows = 0;
+        for (int64_t i = 0; i < ss.n; ++i) max_rows += (ss.s[i]->n + B - 1) / B;
+        SB_TRY(grow(&c.d_multi, &c.multi_cap, (int64_t)(tb + sb + sizeof(int2) * max_rows)));
+        std::vector<StreamEntry> table(ss.n);
+        for (int64_t i = 0; i < ss.n; ++i) table[i] = {ss.s[i]->d_specq, ss.s[i]->nblkq, ss.s[i]->d_raw, ss.s[i]->n, ss.s[i]->d_pfx};
+        multi.d_streams = reinterpret_cast<const StreamEntry*>(c.d_multi);
+        multi.d_slots = reinterpret_cast<const int2*>(c.d_multi + tb);
+        multi.dtype = image->dtype;
+        mp = &multi;
+        std::vector<int2> rows, slots(count);
+        SB_TRY(spectra_rows_multi(ss, count, table.data(), rows));
+        for (int64_t q = 0; q < count; ++q) slots[q] = make_int2(ss.islot[c.h_desc[q].orig], ss.tslot[c.h_desc[q].orig]);
+        int2* d_rows = reinterpret_cast<int2*>(c.d_multi + tb + sb);
+        SB_CUDA(cudaMemcpyAsync(c.d_multi, table.data(), sizeof(StreamEntry) * ss.n, cudaMemcpyHostToDevice, c.stream));
+        SB_CUDA(cudaMemcpyAsync(c.d_multi + tb, slots.data(), sizeof(int2) * count, cudaMemcpyHostToDevice, c.stream));
+        if (!rows.empty()) {
+            SB_CUDA(cudaMemcpyAsync(d_rows, rows.data(), sizeof(int2) * rows.size(), cudaMemcpyHostToDevice, c.stream));
+            ProfScope ps("block_spectra");
+            SB_TRY(launch_block_spectra_quad_multi(multi, d_rows, (int64_t)rows.size()));
+        }
+    } else if (use_packed && n_direct > 0) {
         // spectrum rows the direct class reads: lag block k of a query multiplies rows k .. k+P-1 (a pair: .. k+P)
         int64_t k_lo = INT64_MAX, k_hi = 0;
         for (int64_t q = 0; q < n_direct; ++q) {
@@ -514,7 +600,7 @@ int run_batch(const sb_stream* image_c, const sb_stream* tmpl, int64_t count,
         const int64_t sub = 4096;
         if (use_packed && !premac) {
             ProfScope ps("part_spectra");
-            SB_TRY(launch_part_spectra_quad(tmpl, c.d_desc, (int)qb, (int)qe, part_first, np, c.d_parts));
+            SB_TRY(launch_part_spectra_quad(tmpl, c.d_desc, (int)qb, (int)qe, part_first, np, c.d_parts, mp));
         } else if (use_fused) {                      // hand-written gather + forward FFT, one launch
             ProfScope ps("part_spectra");
             SB_TRY(launch_part_spectra(tmpl, hd, c.d_desc, (int)qb, (int)qe, part_first, np, c.d_parts));
@@ -546,10 +632,10 @@ int run_batch(const sb_stream* image_c, const sb_stream* tmpl, int64_t count,
             if (use_pairs) {
                 const int64_t g0 = c.h_desc[qb].groupBase;
                 const int64_t g1 = (qe < count) ? c.h_desc[qe].groupBase : total_groups;
-                SB_TRY(launch_match_pair(image, tmpl, c.d_parts, part_first, c.d_desc, (int)qb, (int)qe, g0, g1 - g0, c.d_keys, d_curve));
+                SB_TRY(launch_match_pair(image, tmpl, c.d_parts, part_first, c.d_desc, (int)qb, (int)qe, g0, g1 - g0, c.d_keys, d_curve, mp));
             } else
                 SB_TRY(launch_match_packed(image, tmpl, c.d_parts, part_first, c.d_desc, (int)qb, (int)qe,
-                                           item_lo, item_hi - item_lo, c.d_keys, d_curve));
+                                           item_lo, item_hi - item_lo, c.d_keys, d_curve, mp));
         } else if (use_fused && !premac) {
             ProfScope ps("match_fused");
             SB_TRY(launch_match_fused(image, tmpl, hd, c.d_parts, part_first, nullptr, c.d_desc, (int)qb, (int)qe,
@@ -616,6 +702,122 @@ int run_batch(const sb_stream* image_c, const sb_stream* tmpl, int64_t count,
     return SB_OK;
 }
 
+// Queries of `ss` with results to host arrays (sb_find_batch)
+int find_to_host(const StreamSet& ss, int64_t count, const int64_t* tmpl_off, const int64_t* tmpl_len,
+                 const int64_t* lag0, const int64_t* nlags, float* diff_out, int64_t* idx_out) {
+    Ctx& c = ctx();
+    if (c.res_cap < count) {
+        cudaStreamSynchronize(c.stream);
+        cudaFree(c.d_diff); cudaFree(c.d_idx); c.d_diff = nullptr; c.d_idx = nullptr; c.res_cap = 0;
+        SB_CUDA(cudaMalloc(&c.d_diff, sizeof(float) * count));
+        SB_CUDA(cudaMalloc(&c.d_idx, sizeof(int64_t) * count));
+        c.res_cap = count;
+    }
+    if (c.h_res_cap < count) {
+        cudaFreeHost(c.h_diff); cudaFreeHost(c.h_idx); c.h_diff = nullptr; c.h_idx = nullptr; c.h_res_cap = 0;
+        SB_CUDA(cudaMallocHost((void**)&c.h_diff, sizeof(float) * count));
+        SB_CUDA(cudaMallocHost((void**)&c.h_idx, sizeof(int64_t) * count));
+        c.h_res_cap = count;
+    }
+    SB_TRY(run_batch(ss, count, tmpl_off, tmpl_len, lag0, nlags, c.d_diff, c.d_idx, nullptr));
+    SB_CUDA(cudaMemcpyAsync(c.h_diff, c.d_diff, sizeof(float) * count, cudaMemcpyDeviceToHost, c.stream));
+    SB_CUDA(cudaMemcpyAsync(c.h_idx, c.d_idx, sizeof(int64_t) * count, cudaMemcpyDeviceToHost, c.stream));
+    SB_CUDA(cudaStreamSynchronize(c.stream));
+    memcpy(diff_out, c.h_diff, sizeof(float) * count);
+    memcpy(idx_out, c.h_idx, sizeof(int64_t) * count);
+    return SB_OK;
+}
+
+// Whole curves of the queries of `ss`, concatenated in query order, to a host array (sb_match_curves)
+int curves_to_host(const StreamSet& ss, int64_t count, const int64_t* tmpl_off, const int64_t* tmpl_len,
+                   const int64_t* lag0, const int64_t* nlags, float* curves_out) {
+    int64_t total = 0;
+    for (int64_t q = 0; q < count; ++q) total += nlags[q];
+    Ctx& c = ctx();
+    float* d_curve = nullptr; float* d_diff = nullptr; int64_t* d_idx = nullptr;
+    SB_TRY(pool_alloc((void**)&d_curve, sizeof(float) * total));
+    int rc = pool_alloc((void**)&d_diff, sizeof(float) * count);
+    if (rc == SB_OK) rc = pool_alloc((void**)&d_idx, sizeof(int64_t) * count);
+    if (rc == SB_OK) rc = run_batch(ss, count, tmpl_off, tmpl_len, lag0, nlags, d_diff, d_idx, d_curve);
+    if (rc == SB_OK) {
+        cudaError_t e = cudaMemcpyAsync(curves_out, d_curve, sizeof(float) * total, cudaMemcpyDeviceToHost, c.stream);
+        if (e == cudaSuccess) e = cudaStreamSynchronize(c.stream);
+        if (e != cudaSuccess) { set_error("sb_match_curves: D2H: %s", cudaGetErrorString(e)); rc = SB_ECUDA; }
+    }
+    pool_free(d_curve); pool_free(d_diff); pool_free(d_idx);
+    return rc;
+}
+
+// Multi-stream calls.  The packed engine's direct class (engines 2, 4, 5 at B = 16384, hop B; templates below the
+// blocked threshold) goes out as ONE multi-stream batch, whatever the number of streams.  Everything else -- the
+// blocked class, engines 0 / 1, other block sizes, hop B/2 -- runs as one ordinary single-stream batch per distinct
+// (image, template) pair inside the same call: same results, more launches.  Results land in the caller's order.
+int run_multi(const char* who, const sb_stream* const* streams, int32_t n_streams, int64_t count,
+              const int32_t* image_slot, const int32_t* tmpl_slot, const int64_t* tmpl_off, const int64_t* tmpl_len,
+              const int64_t* lag0, const int64_t* nlags, float* diff_out, int64_t* idx_out, float* curves_out) {
+    Ctx& c = ctx();
+    if (!c.inited) SB_FAIL(SB_ESTATE, "%s: library not initialised (call sb_init)", who);
+    if (count < 0) SB_FAIL(SB_EINVAL, "%s: negative count", who);
+    if (count == 0) return SB_OK;
+    if (!streams || n_streams < 1) SB_FAIL(SB_EINVAL, "%s: no streams", who);
+    if (!image_slot || !tmpl_slot || !tmpl_off || !tmpl_len || !lag0 || !nlags || (curves_out ? false : (!diff_out || !idx_out)))
+        SB_FAIL(SB_EINVAL, "%s: NULL array", who);
+    for (int32_t i = 0; i < n_streams; ++i) {
+        if (!streams[i]) SB_FAIL(SB_EINVAL, "%s: stream slot %d is NULL", who, (int)i);
+        if (!streams[i]->d_pfx) SB_FAIL(SB_EINVAL, "%s: stream slot %d has no running sums (a raw sb_load_pcm stream must go through sb_normalise)", who, (int)i);
+        if (streams[i]->dtype != streams[0]->dtype) SB_FAIL(SB_EINVAL, "%s: stream slot %d differs in sample type from slot 0 (all streams of a call share one)", who, (int)i);
+    }
+    for (int64_t q = 0; q < count; ++q) {
+        if (image_slot[q] < 0 || image_slot[q] >= n_streams) SB_FAIL(SB_EINVAL, "%s: query %lld: image slot %d outside [0, %d)", who, (long long)q, (int)image_slot[q], (int)n_streams);
+        if (tmpl_slot[q] < 0 || tmpl_slot[q] >= n_streams) SB_FAIL(SB_EINVAL, "%s: query %lld: template slot %d outside [0, %d)", who, (long long)q, (int)tmpl_slot[q], (int)n_streams);
+        SB_TRY(check_query(streams[image_slot[q]], streams[tmpl_slot[q]], q, tmpl_off[q], tmpl_len[q], lag0[q], nlags[q]));
+    }
+    // run_batch's geometry for these settings: the packed kernels run at hop B unless hop B/2 is forced
+    const bool packed = c.engine >= 2 && packed_supports(c.B) && c.hop_mode != 2;
+    std::vector<int64_t> curve_off(count + 1, 0);
+    for (int64_t q = 0; q < count; ++q) curve_off[q + 1] = curve_off[q] + nlags[q];
+    // one subset of the queries: descriptor arrays gathered, results scattered back to the caller's positions
+    auto run_subset = [&](const std::vector<int64_t>& sel, const StreamSet& ss, std::vector<int32_t>* slots) -> int {
+        const int64_t m = (int64_t)sel.size();
+        std::vector<int64_t> a(4 * m);
+        for (int64_t i = 0; i < m; ++i) {
+            const int64_t q = sel[i];
+            a[i] = tmpl_off[q]; a[m + i] = tmpl_len[q]; a[2 * m + i] = lag0[q]; a[3 * m + i] = nlags[q];
+            if (slots) { slots[0].push_back(image_slot[q]); slots[1].push_back(tmpl_slot[q]); }
+        }
+        StreamSet s2 = ss;
+        if (slots) { s2.islot = slots[0].data(); s2.tslot = slots[1].data(); }
+        if (curves_out && m == count) {        // every query, in the caller's order: straight into the caller's array
+            SB_TRY(curves_to_host(s2, m, &a[0], &a[m], &a[2 * m], &a[3 * m], curves_out));
+        } else if (curves_out) {
+            int64_t total = 0;
+            for (int64_t i = 0; i < m; ++i) total += a[3 * m + i];
+            std::vector<float> cur(total);
+            SB_TRY(curves_to_host(s2, m, &a[0], &a[m], &a[2 * m], &a[3 * m], cur.data()));
+            for (int64_t i = 0, o = 0; i < m; o += a[3 * m + i], ++i) memcpy(curves_out + curve_off[sel[i]], cur.data() + o, sizeof(float) * a[3 * m + i]);
+        } else {
+            std::vector<float> d(m);
+            std::vector<int64_t> k(m);
+            SB_TRY(find_to_host(s2, m, &a[0], &a[m], &a[2 * m], &a[3 * m], d.data(), k.data()));
+            for (int64_t i = 0; i < m; ++i) { diff_out[sel[i]] = d[i]; idx_out[sel[i]] = k[i]; }
+        }
+        return SB_OK;
+    };
+    std::vector<int64_t> direct;
+    std::map<std::pair<int32_t, int32_t>, std::vector<int64_t>> other;
+    for (int64_t q = 0; q < count; ++q) {
+        if (packed && !blocked_class(tmpl_len[q], c.B)) direct.push_back(q);
+        else other[{image_slot[q], tmpl_slot[q]}].push_back(q);
+    }
+    if (!direct.empty()) {
+        StreamSet ss; ss.s = streams; ss.n = n_streams;
+        std::vector<int32_t> slots[2];
+        SB_TRY(run_subset(direct, ss, slots));
+    }
+    for (const auto& g : other) SB_TRY(run_subset(g.second, pair_of(streams[g.first.first], streams[g.first.second]), nullptr));
+    return SB_OK;
+}
+
 int check_common(const char* who, const sb_stream* image, const sb_stream* tmpl, int64_t count) {
     Ctx& c = ctx();
     if (!c.inited) SB_FAIL(SB_ESTATE, "%s: library not initialised (call sb_init)", who);
@@ -636,27 +838,7 @@ int sb_find_batch(const sb_stream* image, const sb_stream* tmpl, int64_t count,
     SB_TRY(check_common("sb_find_batch", image, tmpl, count));
     if (count == 0) return SB_OK;
     if (!tmpl_off || !tmpl_len || !lag0 || !nlags || !diff_out || !idx_out) SB_FAIL(SB_EINVAL, "sb_find_batch: NULL array");
-    Ctx& c = ctx();
-    if (c.res_cap < count) {
-        cudaStreamSynchronize(c.stream);
-        cudaFree(c.d_diff); cudaFree(c.d_idx); c.d_diff = nullptr; c.d_idx = nullptr; c.res_cap = 0;
-        SB_CUDA(cudaMalloc(&c.d_diff, sizeof(float) * count));
-        SB_CUDA(cudaMalloc(&c.d_idx, sizeof(int64_t) * count));
-        c.res_cap = count;
-    }
-    if (c.h_res_cap < count) {
-        cudaFreeHost(c.h_diff); cudaFreeHost(c.h_idx); c.h_diff = nullptr; c.h_idx = nullptr; c.h_res_cap = 0;
-        SB_CUDA(cudaMallocHost((void**)&c.h_diff, sizeof(float) * count));
-        SB_CUDA(cudaMallocHost((void**)&c.h_idx, sizeof(int64_t) * count));
-        c.h_res_cap = count;
-    }
-    SB_TRY(run_batch(image, tmpl, count, tmpl_off, tmpl_len, lag0, nlags, c.d_diff, c.d_idx, nullptr));
-    SB_CUDA(cudaMemcpyAsync(c.h_diff, c.d_diff, sizeof(float) * count, cudaMemcpyDeviceToHost, c.stream));
-    SB_CUDA(cudaMemcpyAsync(c.h_idx, c.d_idx, sizeof(int64_t) * count, cudaMemcpyDeviceToHost, c.stream));
-    SB_CUDA(cudaStreamSynchronize(c.stream));
-    memcpy(diff_out, c.h_diff, sizeof(float) * count);
-    memcpy(idx_out, c.h_idx, sizeof(int64_t) * count);
-    return SB_OK;
+    return find_to_host(pair_of(image, tmpl), count, tmpl_off, tmpl_len, lag0, nlags, diff_out, idx_out);
 }
 
 int sb_find_batch_device(const sb_stream* image, const sb_stream* tmpl, int64_t count,
@@ -666,7 +848,7 @@ int sb_find_batch_device(const sb_stream* image, const sb_stream* tmpl, int64_t 
     SB_TRY(check_common("sb_find_batch_device", image, tmpl, count));
     if (count == 0) return SB_OK;
     if (!tmpl_off || !tmpl_len || !lag0 || !nlags || !d_diff_out || !d_idx_out) SB_FAIL(SB_EINVAL, "sb_find_batch_device: NULL array");
-    return run_batch(image, tmpl, count, tmpl_off, tmpl_len, lag0, nlags, d_diff_out, d_idx_out, nullptr);
+    return run_batch(pair_of(image, tmpl), count, tmpl_off, tmpl_len, lag0, nlags, d_diff_out, d_idx_out, nullptr);
 }
 
 int sb_find(const sb_stream* image, const void* tmpl_host, int64_t tmpl_len,
@@ -688,24 +870,27 @@ int sb_match_curves(const sb_stream* image, const sb_stream* tmpl, int64_t count
     SB_TRY(check_common("sb_match_curves", image, tmpl, count));
     if (count == 0) return SB_OK;
     if (!tmpl_off || !tmpl_len || !lag0 || !nlags || !curves_out) SB_FAIL(SB_EINVAL, "sb_match_curves: NULL array");
-    int64_t total = 0;
-    for (int64_t q = 0; q < count; ++q) {
+    for (int64_t q = 0; q < count; ++q)
         if (nlags[q] < 1) SB_FAIL(SB_EINVAL, "sb_match_curves: query %lld has nlags < 1", (long long)q);
-        total += nlags[q];
-    }
-    Ctx& c = ctx();
-    float* d_curve = nullptr; float* d_diff = nullptr; int64_t* d_idx = nullptr;
-    SB_TRY(pool_alloc((void**)&d_curve, sizeof(float) * total));
-    int rc = pool_alloc((void**)&d_diff, sizeof(float) * count);
-    if (rc == SB_OK) rc = pool_alloc((void**)&d_idx, sizeof(int64_t) * count);
-    if (rc == SB_OK) rc = run_batch(image, tmpl, count, tmpl_off, tmpl_len, lag0, nlags, d_diff, d_idx, d_curve);
-    if (rc == SB_OK) {
-        cudaError_t e = cudaMemcpyAsync(curves_out, d_curve, sizeof(float) * total, cudaMemcpyDeviceToHost, c.stream);
-        if (e == cudaSuccess) e = cudaStreamSynchronize(c.stream);
-        if (e != cudaSuccess) { set_error("sb_match_curves: D2H: %s", cudaGetErrorString(e)); rc = SB_ECUDA; }
-    }
-    pool_free(d_curve); pool_free(d_diff); pool_free(d_idx);
-    return rc;
+    return curves_to_host(pair_of(image, tmpl), count, tmpl_off, tmpl_len, lag0, nlags, curves_out);
+}
+
+int sb_find_multi(const sb_stream* const* streams, int32_t n_streams, int64_t count,
+                  const int32_t* image_slot, const int32_t* tmpl_slot,
+                  const int64_t* tmpl_off, const int64_t* tmpl_len,
+                  const int64_t* lag0, const int64_t* nlags,
+                  float* diff_out, int64_t* idx_out) {
+    return run_multi("sb_find_multi", streams, n_streams, count, image_slot, tmpl_slot, tmpl_off, tmpl_len, lag0, nlags,
+                     diff_out, idx_out, nullptr);
+}
+
+int sb_match_curves_multi(const sb_stream* const* streams, int32_t n_streams, int64_t count,
+                          const int32_t* image_slot, const int32_t* tmpl_slot,
+                          const int64_t* tmpl_off, const int64_t* tmpl_len,
+                          const int64_t* lag0, const int64_t* nlags, float* curves_out) {
+    if (!curves_out && count > 0) SB_FAIL(SB_EINVAL, "sb_match_curves_multi: NULL array");
+    return run_multi("sb_match_curves_multi", streams, n_streams, count, image_slot, tmpl_slot, tmpl_off, tmpl_len, lag0, nlags,
+                     nullptr, nullptr, curves_out);
 }
 
 int sb_match_curve(const sb_stream* image, const sb_stream* tmpl,

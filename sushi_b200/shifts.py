@@ -10,6 +10,13 @@ right half -- sushi.py:445-452) go to the GPU as one batch when the stream suppo
 exactly.  Streams are duck-typed: anything with get_substream /
 find_substream / duration_seconds / sample_rate works (the tests also run this solver on the
 CPU oracle's streams and compare with the reference's golden results).
+
+The solver itself is a generator (_solve) that yields the matcher work it needs and receives the
+answers: a probe triple, or one fast-path search with the speculation that precedes it.
+calculate_shifts answers each request with the stream's own methods, one at a time;
+calculate_shifts_many runs many episodes in lockstep and answers every request that is ready in
+one round -- one multi-stream launch for all probes, one for all speculations -- so the number of
+GPU round trips is the maximum over the episodes instead of their sum.
 """
 import logging
 from itertools import chain
@@ -32,11 +39,25 @@ class _GroupState(object):
             format_time(self.start_time), format_time(self.end_time), self.shift, self.diff))
 
 
-def _probe_triple(dst_stream, audio, left, right, right_offset, center, window):
+# Requests the solver yields (answers in brackets):
+#   ('probe', [q_whole, q_left, q_right])    the three searches of a check  [three (diff, time)]
+#   ('find', q, spec)                        one fast-path search, spec = (groups_list, idx, anchor, window) of the
+#                                            speculation to run first, or None  [(diff, time)]
+# with q = (pattern, center, window), the arguments of find_substream.
+def _answer_alone(src_stream, dst_stream, request):
+    """One request through the stream's own methods, exactly the calls the sequential solver makes."""
+    if request[0] == 'probe':
+        many = getattr(dst_stream, 'find_substream_many', None)
+        return many(request[1]) if many is not None else [dst_stream.find_substream(*q) for q in request[1]]
+    if request[2] is not None:
+        dst_stream.speculate_fast_path(src_stream, *request[2])
+    return dst_stream.find_substream(*request[1])
+
+
+def _probe_triple(audio, left, right, right_offset, center, window):
     """Whole / left-half / right-half search around `center` (sushi.py:450-453)."""
     queries = [(audio, center, window), (left, center, window), (right, center + right_offset, window)]
-    many = getattr(dst_stream, 'find_substream_many', None)
-    results = many(queries) if many is not None else [dst_stream.find_substream(*q) for q in queries]
+    results = yield ('probe', queries)
     diff, whole_time = results[0]
     left_time = results[1][1]
     right_time = results[2][1] - right_offset
@@ -46,6 +67,71 @@ def _probe_triple(dst_stream, audio, left, right, right_offset, center, window):
 
 def calculate_shifts(src_stream, dst_stream, groups_list, normal_window, max_window, rewind_thresh,
                      speculative=True):
+    solver = _solve(src_stream, dst_stream, groups_list, normal_window, max_window, rewind_thresh, speculative)
+    answer = None
+    while True:
+        try:
+            request = solver.send(answer)
+        except StopIteration:
+            return
+        answer = _answer_alone(src_stream, dst_stream, request)
+
+
+def calculate_shifts_many(jobs, normal_window, max_window, rewind_thresh, speculative=True, executor=None):
+    """calculate_shifts over many jobs [(src_stream, dst_stream, groups_list), ...] in lockstep: every job runs on the
+    host until it needs the matcher, then one round answers the requests of all of them, and every job resumes.
+    Per-event results equal running calculate_shifts on each job alone (a value depends only on (template, absolute
+    position), so sharing a launch changes none).  `executor(batch)` answers a round: batch = [(src, dst, request)],
+    returns the answers in order; the default sends all searches out as one sb_find_multi and all speculations as one
+    sb_match_curves_multi.  Returns the number of rounds."""
+    executor = executor or execute_round
+    solvers = [_solve(src, dst, groups, normal_window, max_window, rewind_thresh, speculative) for src, dst, groups in jobs]
+    waiting = {}
+    for j, solver in enumerate(solvers):
+        try:
+            waiting[j] = next(solver)
+        except StopIteration:
+            pass
+    rounds = 0
+    while waiting:
+        order = sorted(waiting)
+        answers = executor([(jobs[j][0], jobs[j][1], waiting[j]) for j in order])
+        rounds += 1
+        for j, answer in zip(order, answers):
+            try:
+                waiting[j] = solvers[j].send(answer)
+            except StopIteration:
+                del waiting[j]
+    return rounds
+
+
+def execute_round(batch):
+    """The default executor of calculate_shifts_many: the speculations of the round from one sb_match_curves_multi
+    (each destination's curve cache filled as speculate_fast_path fills it), then every search of the round -- probe
+    triples and fast-path searches -- from one sb_find_multi; searches a cached curve answers stay on the host.
+    Streams without the multi-stream surface get their requests answered one by one."""
+    from .wavstream import WavStream, find_substreams, speculate_fast_path_many
+    gpu = [isinstance(dst, WavStream) for _, dst, _ in batch]
+    speculations = [(dst, src) + tuple(req[2]) for (src, dst, req), g in zip(batch, gpu) if g and req[0] == 'find' and req[2]]
+    if speculations:
+        speculate_fast_path_many(speculations)
+    searches = []
+    for (src, dst, req), g in zip(batch, gpu):
+        if g:
+            searches += [(dst,) + tuple(q) for q in (req[1] if req[0] == 'probe' else [req[1]])]
+    found = iter(find_substreams(searches))
+    answers = []
+    for (src, dst, req), g in zip(batch, gpu):
+        if not g:
+            answers.append(_answer_alone(src, dst, req))
+        elif req[0] == 'probe':
+            answers.append([next(found) for _ in req[1]])
+        else:
+            answers.append(next(found))
+    return answers
+
+
+def _solve(src_stream, dst_stream, groups_list, normal_window, max_window, rewind_thresh, speculative):
     committed, pending = [], []
     # streams that can precompute the coming fast-path searches in one launch expose this hook; the
     # results they then return are the ones a live call would return (see WavStream.speculate_fast_path)
@@ -68,9 +154,8 @@ def calculate_shifts(src_stream, dst_stream, groups_list, normal_window, max_win
                     logging.info('{0}-{1}: outside of audio range'.format(format_time(rest[0].start), format_time(rest[-1].end)))
                 break
             if SMALL_WINDOW < window:
-                if speculate is not None:
-                    speculate(src_stream, groups_list, idx, anchor, SMALL_WINDOW)
-                diff, found = dst_stream.find_substream(audio, origin + anchor, SMALL_WINDOW)
+                spec = (groups_list, idx, anchor, SMALL_WINDOW) if speculate is not None else None
+                diff, found = yield ('find', (audio, origin + anchor, SMALL_WINDOW), spec)
             if found is not None and abs((found - origin) - anchor) <= ALLOWED_ERROR:
                 # the shift did not move: commit straight away (sushi.py:434-443)
                 state.shift, state.diff = found - origin, diff
@@ -93,8 +178,8 @@ def calculate_shifts(src_stream, dst_stream, groups_list, normal_window, max_win
                 continue
             if not origin + center_shift < dst_stream.duration_seconds:
                 continue
-            diff, found, left_time, right_time, agreed = _probe_triple(
-                dst_stream, audio, left, right, right_offset, origin + center_shift, window)
+            diff, found, left_time, right_time, agreed = yield from _probe_triple(
+                audio, left, right, right_offset, origin + center_shift, window)
             logging.debug('{0}-{1}: shift: {2:0.5f} [{3:0.5f}, {4:0.5f}], search offset: {5:0.6f}'.format(
                 format_time(state.start_time), format_time(state.end_time), found - origin,
                 left_time - origin, right_time - origin, center_shift))

@@ -564,6 +564,13 @@ class WavStream(StreamGeometry):
         contained range with exactly the value and first-index argmin a live call returns (the packed
         engines at hop B, the default, compute a value the same way whatever the batch; the
         first-generation engine with hop_mode 0 picks its geometry per batch and agrees only to ~1e-7)."""
+        plan = self._speculation_plan(src_stream, groups, idx, anchor, window)
+        if plan is not None:
+            self._fill_curve_cache(src_stream, plan, self.match_curves(src_stream, *plan))
+
+    def _speculation_plan(self, src_stream, groups, idx, anchor, window):
+        """The queries speculate_fast_path would precompute, (toff, tlen, lag0, nlags), or None when the cache already
+        holds the group's curve or no group fits its search span."""
         cache = self.__dict__.setdefault('_curve_cache', {})
         # keys are the CLAMPED template ranges, the same integers find_substream derives from a view.  This runs once
         # per search group: the common case (the group's curve is there) must cost a few scalar operations, not arrays
@@ -575,7 +582,7 @@ class WavStream(StreamGeometry):
             lo = max(lo + total, 0) if lo < 0 else min(lo, total)
             hi = max(hi + total, 0) if hi < 0 else min(hi, total)
             if (lo, lo + max(hi - lo, 0)) in cache:
-                return
+                return None
         batch = groups[idx:idx + self.SPECULATE_GROUPS]
         starts = np.array([g[0].start for g in batch], np.float64)
         ends = np.array([g[-1].end for g in batch], np.float64)
@@ -593,10 +600,14 @@ class WavStream(StreamGeometry):
                 except SushiError:
                     pass
             if not keep:
-                return
+                return None
             toff, tlen, lag0, nlags, _ = self.plan_queries(src_stream, starts[keep], ends[keep], starts[keep] + anchor,
                                                            windows[keep])
-        curves = self.match_curves(src_stream, toff, tlen, lag0, nlags)
+        return toff, tlen, lag0, nlags
+
+    def _fill_curve_cache(self, src_stream, plan, curves):
+        toff, tlen, lag0, _ = plan
+        cache = self.__dict__.setdefault('_curve_cache', {})
         for q in range(len(toff)):
             cache[(int(toff[q]), int(toff[q] + tlen[q]))] = (src_stream, int(lag0[q]), curves[q])
 
@@ -621,3 +632,110 @@ class WavStream(StreamGeometry):
         _native.check(self._lib.sb_match_curve(self._handle, src_stream._handle, int(toff), int(tlen), int(lag0),
                                                int(nlags), out.ctypes.data_as(_native.c_f32p)), 'sb_match_curve')
         return out
+
+
+# -- many streams at once (sb_find_multi / sb_match_curves_multi) ---------------------------------
+def _multi_arrays(pairs):
+    """[(image_stream, tmpl_stream), ...] -> (stream table, image slots, template slots) of one multi-stream call."""
+    slot, handles = {}, []
+    islot = np.empty(len(pairs), np.int32)
+    tslot = np.empty(len(pairs), np.int32)
+    for q, (img, tmpl) in enumerate(pairs):
+        for s, out in ((img, islot), (tmpl, tslot)):
+            if id(s) not in slot:
+                slot[id(s)] = len(handles)
+                handles.append(s._handle)
+            out[q] = slot[id(s)]
+    table = (ctypes.c_void_p * len(handles))(*[h.value for h in handles])
+    return table, len(handles), islot, tslot
+
+
+def _by_dtype(items, key):
+    groups = {}
+    for i, it in enumerate(items):
+        groups.setdefault(key(it), []).append(i)
+    return groups.values()
+
+
+def find_substreams(requests):
+    """[(dst_stream, pattern, window_center, window_size), ...] -> [(np.float32, float), ...]: for every request exactly
+    what dst_stream.find_substream(pattern, window_center, window_size) returns.  Requests whose pattern is a view of a
+    live stream go out together in ONE sb_find_multi per sample type, whatever their streams (a curve cached by
+    speculate_fast_path answers on the host, as in find_substream); anything else -- detached copies, a search span
+    shorter than the pattern -- goes through dst_stream.find_substream."""
+    out = [None] * len(requests)
+    live = []
+    for r, (dst, pattern, center, window) in enumerate(requests):
+        where = dst._locate(pattern) if pattern.dtype == dst.data.dtype else None
+        n = len(pattern[0])
+        start_time, lo, span = dst._window(n, center, window)
+        if where is None or n < 1 or span < n:
+            out[r] = dst.find_substream(pattern, center, window)
+            continue
+        cached = dst._from_cache(where, n, lo, span - n + 1)
+        if cached is not None:
+            out[r] = (np.float32(cached[0]), start_time + (cached[1] / float(dst.sample_rate)))
+            continue
+        live.append((r, dst, where[0], where[1], n, lo, span - n + 1, start_time))
+    for sel in _by_dtype(live, lambda x: x[1].data.dtype):
+        part = [live[i] for i in sel]
+        table, n_streams, islot, tslot = _multi_arrays([(x[1], x[2]) for x in part])
+        arrs = [np.ascontiguousarray([x[k] for x in part], dtype=np.int64) for k in (3, 4, 5, 6)]
+        diff = np.empty(len(part), np.float32)
+        idx = np.empty(len(part), np.int64)
+        lib = part[0][1]._lib
+        _native.check(lib.sb_find_multi(table, n_streams, len(part), islot.ctypes.data_as(_native.c_i32p),
+                                        tslot.ctypes.data_as(_native.c_i32p), *[a.ctypes.data_as(_native.c_i64p) for a in arrs],
+                                        diff.ctypes.data_as(_native.c_f32p), idx.ctypes.data_as(_native.c_i64p)), 'sb_find_multi')
+        for q, x in enumerate(part):
+            out[x[0]] = (np.float32(diff[q]), x[7] + (int(idx[q]) / float(x[1].sample_rate)))
+    return out
+
+
+def match_curves_multi(requests):
+    """[(dst_stream, src_stream, toff, tlen, lag0, nlags), ...] with descriptor arrays per request -> per request the list
+    of curves dst_stream.match_curves(src_stream, toff, tlen, lag0, nlags) returns; one sb_match_curves_multi per
+    sample type."""
+    out = [None] * len(requests)
+    for sel in _by_dtype(requests, lambda r: r[0].data.dtype):
+        pairs, cols, counts = [], [[], [], [], []], []
+        for i in sel:
+            dst, src, toff, tlen, lag0, nlags = requests[i]
+            counts.append(len(toff))
+            pairs += [(dst, src)] * len(toff)
+            for k, a in enumerate((toff, tlen, lag0, nlags)):
+                cols[k] += [int(v) for v in a]
+        if not pairs:
+            for i in sel:
+                out[i] = []
+            continue
+        table, n_streams, islot, tslot = _multi_arrays(pairs)
+        arrs = [np.ascontiguousarray(c, dtype=np.int64) for c in cols]
+        curves = np.empty(int(arrs[3].sum()), np.float32)
+        lib = requests[sel[0]][0]._lib
+        _native.check(lib.sb_match_curves_multi(table, n_streams, len(pairs), islot.ctypes.data_as(_native.c_i32p),
+                                                tslot.ctypes.data_as(_native.c_i32p), *[a.ctypes.data_as(_native.c_i64p) for a in arrs],
+                                                curves.ctypes.data_as(_native.c_f32p)), 'sb_match_curves_multi')
+        pieces = np.split(curves, np.cumsum(arrs[3])[:-1])
+        at = 0
+        for i, cnt in zip(sel, counts):
+            out[i] = pieces[at:at + cnt]
+            at += cnt
+    return out
+
+
+def speculate_fast_path_many(requests):
+    """[(dst_stream, src_stream, groups, idx, anchor, window), ...]: speculate_fast_path for every request, with the
+    curves of all of them from ONE sb_match_curves_multi.  Each destination's cache is filled, keyed exactly like
+    speculate_fast_path's; two requests on one destination evict each other's entries (later live calls are slower,
+    never different)."""
+    todo = []
+    for dst, src, groups, idx, anchor, window in requests:
+        plan = dst._speculation_plan(src, groups, idx, anchor, window)
+        if plan is not None:
+            todo.append((dst, src, plan))
+    if not todo:
+        return
+    curves = match_curves_multi([(dst, src) + tuple(plan) for dst, src, plan in todo])
+    for (dst, src, plan), c in zip(todo, curves):
+        dst._fill_curve_cache(src, plan, c)
