@@ -1,11 +1,13 @@
-"""The grouping heuristics that sit either side of the matcher (reference sushi.py:67-216,309-397).
-They decide which events are correlated (search groups) and post-process the (shift, diff) pairs the
-matcher returns.  Behaviour follows the reference function for function; the reference's own unit
-tests for them (tests/main.py:34-165) are ported in tests/test_grouping.py.
+"""The grouping heuristics that sit either side of the matcher (reference sushi.py:67-397).
+They decide which events are correlated (search groups), post-process the (shift, diff) pairs the
+matcher returns and, when keyframes are given, correct the result against video keyframes.
+Behaviour follows the reference function for function; the reference's own unit tests for them
+(tests/main.py:34-181) are ported in tests/test_grouping.py and tests/test_timing.py.
 
 Events are duck-typed: anything with start/end/shift/diff/linked and set_shift/link_event works
 (ScriptEvent here, subs.ScriptEventBase in the reference, FakeEvent in its tests).
 """
+import bisect
 import logging
 
 import numpy as np
@@ -214,6 +216,99 @@ def merge_short_lines_into_groups(events, chapter_times, max_ts_duration, max_ts
             i += 1
         groups.append(group)
     return groups
+
+
+def get_distance_to_closest_kf(timestamp, keyframes):
+    """Signed distance from `timestamp` to the nearest keyframe time; ties go to the earlier one (sushi.py:218-228)."""
+    idx = bisect.bisect_left(keyframes, timestamp)
+    if idx == 0:
+        kf = keyframes[0]
+    elif idx == len(keyframes):
+        kf = keyframes[-1]
+    else:
+        before, after = keyframes[idx - 1], keyframes[idx]
+        kf = after if after - timestamp < timestamp - before else before
+    return kf - timestamp
+
+
+def find_keyframe_shift(group, src_keytimes, dst_keytimes, src_timecodes, dst_timecodes, max_kf_distance):
+    """(start, end) corrections that put a search group's edges on the destination keyframes matching
+    the source ones, None where no keyframe pair is within reach (sushi.py:231-248)."""
+    def get_distance(src_distance, dst_distance, limit):
+        if abs(dst_distance) > limit:
+            return None
+        shift = dst_distance - src_distance
+        return shift if abs(shift) < limit else None
+
+    src_start = get_distance_to_closest_kf(group[0].start, src_keytimes)
+    src_end = get_distance_to_closest_kf(group[-1].end + src_timecodes.get_frame_size(group[-1].end), src_keytimes)
+    dst_start = get_distance_to_closest_kf(group[0].shifted_start, dst_keytimes)
+    # the frame size is looked up at the UNSHIFTED end on the destination timecodes (sushi.py:242)
+    dst_end = get_distance_to_closest_kf(group[-1].shifted_end + dst_timecodes.get_frame_size(group[-1].end), dst_keytimes)
+    snapping_limit_start = src_timecodes.get_frame_size(group[0].start) * max_kf_distance
+    snapping_limit_end = src_timecodes.get_frame_size(group[0].end) * max_kf_distance    # group[0], not group[-1] (sushi.py:245)
+    return (get_distance(src_start, dst_start, snapping_limit_start),
+            get_distance(src_end, dst_end, snapping_limit_end))
+
+
+def find_keyframes_distances(event, src_keytimes, dst_keytimes, timecodes, max_kf_distance):
+    """Separate start / end corrections of one event when both its source and shifted times sit
+    near keyframes (sushi.py:251-263)."""
+    def find_keyframe_distance(src_time, dst_time):
+        src = get_distance_to_closest_kf(src_time, src_keytimes)
+        dst = get_distance_to_closest_kf(dst_time, dst_keytimes)
+        snapping_limit = timecodes.get_frame_size(src_time) * max_kf_distance
+        if abs(src) < snapping_limit and abs(dst) < snapping_limit and abs(src - dst) < snapping_limit:
+            return dst - src
+        return 0
+
+    return find_keyframe_distance(event.start, event.shifted_start), find_keyframe_distance(event.end, event.shifted_end)
+
+
+def snap_groups_to_keyframes(events, chapter_times, max_ts_duration, max_ts_distance, src_keytimes, dst_keytimes,
+                             src_timecodes, dst_timecodes, max_kf_distance, kf_mode):
+    """Keyframe correction of already shifted, unlinked events (sushi.py:266-306).  Step 1 ('shift' /
+    'all') moves every search group by its keyframe correction, keeping durations; step 2 ('snap' /
+    'all') moves the start and end of each group's first event onto nearby keyframes."""
+    if not max_kf_distance:
+        return
+    groups = merge_short_lines_into_groups(events, chapter_times, max_ts_duration, max_ts_distance)
+
+    if kf_mode == 'all' or kf_mode == 'shift':
+        shifts, times = [], []
+        for group in groups:
+            shifts.extend(find_keyframe_shift(group, src_keytimes, dst_keytimes, src_timecodes, dst_timecodes,
+                                              max_kf_distance))
+            times.extend((group[0].shifted_start, group[-1].shifted_end))
+        shifts = interpolate_nones(shifts, times)
+        if shifts:
+            mean_shift = np.mean(shifts)
+            pairs = zip(*(iter(shifts),) * 2)
+            logging.info('Group {0}-{1} corrected by {2}'.format(format_time(events[0].start), format_time(events[-1].end),
+                                                                 mean_shift))
+            for group, (start_shift, end_shift) in zip(groups, pairs):
+                if abs(start_shift - end_shift) > 0.001 and len(group) > 1:
+                    # on a tie min() keeps the start shift
+                    actual_shift = min(start_shift, end_shift, key=lambda x: abs(x - mean_shift))
+                    logging.warning('Typesetting group at {0} had different shift at start/end points ({1} and {2}). '
+                                    'Shifting by {3}.'.format(format_time(group[0].start), start_shift, end_shift,
+                                                              actual_shift))
+                    for e in group:
+                        e.adjust_shift(actual_shift)
+                else:
+                    for e in group:
+                        e.adjust_additional_shifts(start_shift, end_shift)
+
+    if kf_mode == 'all' or kf_mode == 'snap':
+        # the reference means to leave typesetting groups alone here but its check is a no-op
+        # (sushi.py:301-302): every group's first event is snapped
+        for group in groups:
+            start_shift, end_shift = find_keyframes_distances(group[0], src_keytimes, dst_keytimes, src_timecodes,
+                                                              max_kf_distance)
+            if abs(start_shift) > 0.01 or abs(end_shift) > 0.01:
+                logging.info('Snapping {0} to keyframes, start time by {1}, end: {2}'.format(
+                    format_time(group[0].start), start_shift, end_shift))
+                group[0].adjust_additional_shifts(start_shift, end_shift)
 
 
 def prepare_search_groups(events, source_duration, chapter_times, max_ts_duration, max_ts_distance):
