@@ -74,9 +74,10 @@ def readframes(raw, sample_width, channels):          # wav.py:64-91
     return data
 
 
-def load_stream(read_raw, frames_count, framerate, sample_width, channels, sample_rate=12000, sample_type='uint8'):
-    """wav.py:108-156 with `read_raw(nframes) -> bytes` standing in for the open file.
-    Returns (data (1,N), sample_count, padding_size)."""
+def pad_stream(read_raw, frames_count, framerate, sample_width, channels, sample_rate=12000, skip_empty=False):
+    """wav.py:108-141: the chunk loop and the edge padding, before normalisation.
+    Returns (padded float32 data (1,N), sample_count, padding_size).  skip_empty=True is NOT the reference: a read
+    that resamples to no sample, where cv2.resize raises, contributes none (the product's documented rule)."""
     total_seconds = frames_count / float(framerate)
     downsample_rate = sample_rate / float(framerate)
     sample_count = math.ceil(total_seconds * sample_rate)
@@ -88,6 +89,9 @@ def load_stream(read_raw, frames_count, framerate, sample_width, channels, sampl
     while seconds_read < total_seconds:
         chunk = readframes(read_raw(int(1 * framerate)), sample_width, channels)
         new_length = int(_py2_round(len(chunk) * downsample_rate))
+        if skip_empty and new_length == 0:
+            seconds_read += 1
+            continue
         dst_view = data[0][samples_read:samples_read + new_length]
         if downsample_rate != 1:
             chunk = chunk.reshape((1, len(chunk)))
@@ -97,6 +101,11 @@ def load_stream(read_raw, frames_count, framerate, sample_width, channels, sampl
         seconds_read += 1
     data[0][0:padding_size].fill(data[0][padding_size])
     data[0][-padding_size:].fill(data[0][-padding_size - 1])
+    return data, sample_count, padding_size
+
+
+def normalise(data, sample_type='uint8'):
+    """wav.py:145-156 on a padded array (overwritten).  Returns (data, min_value, max_value)."""
     max_value = np.median(data[data >= 0], overwrite_input=True) * 3
     min_value = np.median(data[data <= 0], overwrite_input=True) * 3
     np.clip(data, min_value, max_value, out=data)
@@ -106,7 +115,23 @@ def load_stream(read_raw, frames_count, framerate, sample_width, channels, sampl
         data *= 255.0
         data += 0.5
         data = data.astype('uint8')
+    return data, min_value, max_value
+
+
+def load_stream(read_raw, frames_count, framerate, sample_width, channels, sample_rate=12000, sample_type='uint8'):
+    """wav.py:108-156 with `read_raw(nframes) -> bytes` standing in for the open file.
+    Returns (data (1,N), sample_count, padding_size)."""
+    data, sample_count, padding_size = pad_stream(read_raw, frames_count, framerate, sample_width, channels, sample_rate)
+    data, _, _ = normalise(data, sample_type)
     return data, sample_count, padding_size
+
+
+def load_wav_padded(path, sample_rate=12000):
+    """(padded float32 data before normalisation, sample_count, padding_size) of a WAV file."""
+    with open(path, 'rb') as f:
+        info = parse_header(f, path)
+        return pad_stream(lambda n: f.read(n * info['frame_size']), info['frames_count'], info['framerate'],
+                          info['sample_width'], info['channels'], sample_rate)
 
 
 def load_wav(path, sample_rate=12000, sample_type='uint8'):

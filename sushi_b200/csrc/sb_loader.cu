@@ -27,7 +27,7 @@ struct ResampleGeom {
     double ifx_last;
     int64_t padding;       // wav.py:120
     int64_t total;         // wav.py:119
-    int64_t written;       // samples produced by the chunk loop
+    int64_t written;       // samples produced by the chunk loop (may run past total - padding: see sb_load_pcm)
 };
 
 // One frame -> the integer numerator of the reference's float32 sample: int16 values (int24: bytes 1,2,
@@ -87,7 +87,7 @@ k_decode_resample_pad(const unsigned char* __restrict__ pcm, ResampleGeom g, Loa
 #pragma unroll
             for (int r = 0; r < 4; ++r) {
                 const int x = slab * 1024 + r * 256 + threadIdx.x;
-                if (x < outn) {
+                if (x < outn && o0 + x < tail0) {                         // what lands in the tail padding is overwritten
                     int sx = x;
                     if (g.resample) { sx = (int)floor((double)x * ifx); if (sx > len - 1) sx = len - 1; }   // OpenCV resizeNN: cvFloor(x * ifx)
                     const int acc = decode_acc(pcm, frame0 + sx, channels, width);
@@ -319,8 +319,12 @@ int sb_load_pcm(const void* pcm_host, int64_t frames, int channels, int sample_w
     g.ifx_last = (g.out_last > 0 && g.len_last > 0) ? 1.0 / ((double)g.out_last / (double)g.len_last) : 0.0;
     g.padding = padding; g.total = total_len;
     g.written = g.nfull * (int64_t)g.out_full + g.out_last;
+    // The reference reads whole seconds from the start of the data chunk (wav.py:125-137), so `frames` may hold more
+    // than the total_len - 2 * padding samples the header accounts for (a chunk after the PCM) or fewer (a truncated
+    // file).  Samples past the content region are overwritten by the tail padding there and are not written here;
+    // samples past the end of the buffer make the reference's copy fail.
     if (g.written > total_len - padding)
-        SB_FAIL(SB_EINVAL, "sb_load_pcm: %lld resampled samples do not fit a buffer of %lld with %lld padding",
+        SB_FAIL(SB_EINVAL, "sb_load_pcm: %lld resampled samples run past a buffer of %lld with %lld padding",
                 (long long)g.written, (long long)total_len, (long long)padding);
 
     if (channels > kMaxChannels) SB_FAIL(SB_EINVAL, "sb_load_pcm: %d channels (at most %d)", channels, kMaxChannels);

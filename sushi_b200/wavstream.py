@@ -233,7 +233,10 @@ class WavStream(StreamGeometry):
         stream = DownmixedWavFile(path)
         try:
             if loader == 'gpu':
-                pcm = stream.read_raw(stream.frames_count)
+                # what the reference's chunk loop reads (wav.py:125-137): whole seconds from the start of the data
+                # chunk, so the last read can run past the chunk or stop short at the end of a truncated file
+                reads = math.ceil(stream.frames_count / float(stream.framerate))
+                pcm = stream.read_raw(reads * stream.framerate)
                 self._load_gpu(pcm, stream.frames_count, stream.channels_count, stream.sample_width,
                                stream.framerate, sample_rate, sample_type, device)
             else:
@@ -249,10 +252,12 @@ class WavStream(StreamGeometry):
 
     def _load_gpu(self, pcm, frames, channels, sample_width, framerate, sample_rate, sample_type, device):
         """wav.py:108-156 on the GPU: geometry here (same scalar code as the reference), arithmetic
-        in sb_load_pcm / sb_normalise; .data is then mirrored back for get_substream views."""
+        in sb_load_pcm / sb_normalise; .data is then mirrored back for get_substream views.  `frames` is the
+        header's frame count, which sizes the stream; `pcm` is every byte the chunk loop reads, which may be more or
+        fewer frames (a partial frame at its end is dropped, as readframes drops it)."""
         if sample_width not in (2, 3):
             raise SushiError('Unsupported sample width: {0}'.format(sample_width))
-        frames = min(frames, len(pcm) // (channels * sample_width))
+        decoded = len(pcm) // (channels * sample_width)
         total_seconds = frames / float(framerate)
         self.sample_count = math.ceil(total_seconds * sample_rate)
         self.sample_rate = sample_rate
@@ -261,9 +266,9 @@ class WavStream(StreamGeometry):
         total = int(self.PADDING_SECONDS * 2 * framerate + self.sample_count)
         lib = _native.lib(device)
         raw = ctypes.c_void_p()
-        buf = np.frombuffer(pcm, dtype=np.uint8)
+        buf = np.frombuffer(pcm, dtype=np.uint8, count=decoded * channels * sample_width)
         with nvtx_range('sushi_b200: sb_load_pcm'):
-            _native.check(lib.sb_load_pcm(buf.ctypes.data_as(ctypes.c_void_p), frames, channels, sample_width,
+            _native.check(lib.sb_load_pcm(buf.ctypes.data_as(ctypes.c_void_p), decoded, channels, sample_width,
                                           framerate, sample_rate, self.padding_size, total, ctypes.byref(raw)), 'sb_load_pcm')
         h = ctypes.c_void_p()
         lo, hi = ctypes.c_float(), ctypes.c_float()
@@ -300,7 +305,11 @@ class WavStream(StreamGeometry):
         while seconds_read < total_seconds:
             mono = stream.readframes(chunk_frames)
             new_length = int(py2_round(len(mono) * downsample_rate))
-            if downsample_rate != 1 and len(mono):
+            if not new_length:
+                # a last chunk too short for one output sample: the reference's cv2.resize raises here; this
+                # loader, like the GPU one, takes no sample from it (DESIGN.md section 2)
+                mono = mono[:0]
+            elif downsample_rate != 1:
                 key = (len(mono), new_length)
                 if key not in maps:
                     maps[key] = nearest_index_map(*key)
