@@ -1193,15 +1193,18 @@ __global__ void k_fill_pair_query(const QueryDesc* __restrict__ desc, int q_begi
 // Same transform as k_forward_rows in sb_fused.cu (gather + centring + 2B-point real FFT through the
 // shared-memory inverse passes run backwards); only the output stage differs: bins leave as the chunks
 // A[i] = (X[i], X[i+B/2]) and M[i] = (X[B-i], X[B/2-i]) the packed kernel multiplies.
-// MULTI: MODE 0 builds the rows row_list[blockIdx.x] = (slot, row) of several streams, each into its own stream's
-// rows; MODE 1 reads every query's template from its template slot.
+// MULTI: MODE 0 builds the rows row_list[i] = (slot, row) of several streams, each into its own stream's rows; MODE 1
+// reads every query's template from its template slot.
+// Persistent: a CTA walks the launch's rows i = blockIdx.x, + gridDim.x, .. < rows, so the FFT's twiddle tables
+// travel to shared memory once per CTA (rows < 0: the CTA builds row blockIdx.x only, a launch of one CTA per row).  In MODE 1 a row's query is found by the whole CTA, 512 descriptors per step
+// (two steps of dependent loads for up to 262 144 queries instead of one thread's binary search).
 template <typename S, int MODE, bool MULTI = false>
 __global__ void __launch_bounds__(Cfg<14>::T, 1)
 k_forward_quad(const S* __restrict__ src, int64_t src_n, const double2* __restrict__ pfx,
                const QueryDesc* __restrict__ desc, int q_begin, int q_end, int64_t row_first,
                FusedTables tab, float4* __restrict__ out,
                const StreamEntry* __restrict__ streams = nullptr, const int2* __restrict__ slots = nullptr,
-               const int2* __restrict__ row_list = nullptr) {
+               const int2* __restrict__ row_list = nullptr, int64_t rows = -1) {
     typedef Cfg<14> C;
     constexpr int N = C::N, T = C::T, B = C::N;
     constexpr int NT2 = C::R2 * 32, NT3 = C::R3 * 32;
@@ -1210,69 +1213,88 @@ k_forward_quad(const S* __restrict__ src, int64_t src_n, const double2* __restri
     float2* s_t2 = buf + pad(N) + 1;
     float2* s_a3 = s_t2 + NT2;
     float2* s_b3 = s_a3 + NT3;
-    __shared__ int s_q;
+    int* s_q = reinterpret_cast<int*>(s_b3 + NT3);           // in the 64 bytes behind the tables
     const int tid = threadIdx.x;
     for (int i = tid; i < NT2; i += T) s_t2[i] = __ldg(tab.t2 + i);
     for (int i = tid; i < NT3; i += T) { s_a3[i] = __ldg(tab.a3 + i); s_b3[i] = __ldg(tab.b3 + i); }
 
-    int64_t off, len;          // samples [off, off+len) of src, zero beyond
-    float centre;
-    int64_t row = row_first + blockIdx.x, out_row = blockIdx.x;
-    if constexpr (MULTI && MODE == 0) {
-        const int2 rl = row_list[blockIdx.x];
-        const StreamEntry se = streams[rl.x];
-        src = static_cast<const S*>(se.raw); src_n = se.n; pfx = se.pfx;
-        out = reinterpret_cast<float4*>(se.specq);
-        row = out_row = rl.y;
-    }
-    if (MODE == 0) {
-        off = row * B;
-        len = src_n - off; if (len > 2 * B) len = 2 * B; if (len < 0) len = 0;
-        centre = Acc<S>::centre(pfx[src_n].x, (double)src_n);
-    } else {
-        if (tid == 0) {        // largest q with partBase <= row
-            int lo = q_begin, hi = q_end - 1;
-            while (lo < hi) { int mid = (lo + hi + 1) >> 1; if (desc[mid].partBase <= row) lo = mid; else hi = mid - 1; }
-            s_q = lo;
+    for (int64_t item = blockIdx.x; rows < 0 ? item == blockIdx.x : item < rows; item += gridDim.x) {
+        const S* xs = src;
+        const double2* xpfx = pfx;
+        float4* xout = out;
+        int64_t off, len;          // samples [off, off+len) of xs, zero beyond
+        float centre;
+        int64_t row = row_first + item, out_row = item;
+        if constexpr (MULTI && MODE == 0) {
+            const int2 rl = row_list[item];
+            const StreamEntry se = streams[rl.x];
+            xs = static_cast<const S*>(se.raw); xpfx = se.pfx;
+            xout = reinterpret_cast<float4*>(se.specq);
+            row = out_row = rl.y;
+            off = row * B;
+            len = se.n - off; if (len > 2 * B) len = 2 * B; if (len < 0) len = 0;
+            centre = Acc<S>::centre(xpfx[se.n].x, (double)se.n);
+        } else if (MODE == 0) {
+            off = row * B;
+            len = src_n - off; if (len > 2 * B) len = 2 * B; if (len < 0) len = 0;
+            centre = Acc<S>::centre(pfx[src_n].x, (double)src_n);
+        } else {
+            // largest q in [q_begin, q_end) with partBase <= row: each step tests the candidates lo + t*s, t < m, and the
+            // one thread whose candidate is the last that passes writes its t
+            int lo = q_begin, n = q_end - q_begin;
+            while (n > 1) {
+                const int s = (n + T - 1) / T, m = (n + s - 1) / s;
+                auto le = [&](int t) { return t == 0 || (t < m && desc[lo + t * s].partBase <= row); };
+                if (le(tid) && !le(tid + 1)) *s_q = tid;
+                __syncthreads();
+                const int c = *s_q;
+                __syncthreads();            // s_q is written again by the next step
+                lo += c * s;
+                n = c == m - 1 ? n - c * s : s;
+            }
+            const int q = lo;
+            const QueryDesc d = desc[q];
+            if constexpr (MULTI) { xs = static_cast<const S*>(streams[slots[q].y].raw); xpfx = streams[slots[q].y].pfx; }
+            const int64_t seg0 = (row - d.partBase) * B;
+            off = d.toff + seg0;
+            len = d.tlen - seg0; if (len > B) len = B;
+            centre = Acc<S>::centre(xpfx[d.toff + d.tlen].x - xpfx[d.toff].x, (double)d.tlen);
+        }
+        const S* x = xs + off;
+        // all 64 sample loads of a thread in flight at once (the previous row's output stage has read buf: the barrier
+        // at the end of the loop body)
+#pragma unroll
+        for (int k = 0; k < B / T; ++k) {
+            const int n = tid + k * T;
+            const int64_t i0 = 2 * (int64_t)n;
+            const float a = i0 < len ? (float)x[i0] - centre : 0.f;
+            const float b = i0 + 1 < len ? (float)x[i0 + 1] - centre : 0.f;
+            buf[pad(n)] = make_float2(a, -b);            // conj(z[n])
         }
         __syncthreads();
-        const QueryDesc d = desc[s_q];
-        if constexpr (MULTI) { src = static_cast<const S*>(streams[slots[s_q].y].raw); pfx = streams[slots[s_q].y].pfx; }
-        const int64_t seg0 = (row - d.partBase) * B;
-        off = d.toff + seg0;
-        len = d.tlen - seg0; if (len > B) len = B;
-        centre = Acc<S>::centre(pfx[d.toff + d.tlen].x - pfx[d.toff].x, (double)d.tlen);
-    }
-    const S* x = src + off;
-#pragma unroll 4
-    for (int n = tid; n < B; n += T) {
-        const int64_t i0 = 2 * (int64_t)n;
-        const float a = i0 < len ? (float)x[i0] - centre : 0.f;
-        const float b = i0 + 1 < len ? (float)x[i0 + 1] - centre : 0.f;
-        buf[pad(n)] = make_float2(a, -b);            // conj(z[n])
-    }
-    __syncthreads();
-    ifft_smem<14, C::R3, false>(buf, s_t2, s_a3, s_b3);   // buf = conj(Z)
-    // bins k and B-k from Z[k], Z[B-k]:  X[k] = Xe + conj(w^k)*Xo,  X[B-k] = conj(Xe - conj(w^k)*Xo)
-    auto bins = [&](int k, float2& xk, float2& xbk) {
-        const float2 zk = buf[pad(k)];
-        const float2 zp = buf[pad(k == 0 ? 0 : B - k)];
-        const float2 A = make_float2(zk.x, -zk.y), P = make_float2(zp.x, zp.y);     // Z[k], conj(Z[B-k])
-        const float2 xe = make_float2(0.5f * (A.x + P.x), 0.5f * (A.y + P.y));
-        const float2 dd = make_float2(A.x - P.x, A.y - P.y);
-        const float2 xo = make_float2(0.5f * dd.y, -0.5f * dd.x);                   // -i*dd/2
-        const float2 w = __ldg(tab.w + k);
-        const float2 tv = cmul(make_float2(w.x, -w.y), xo);
-        xk = make_float2(xe.x + tv.x, xe.y + tv.y);
-        xbk = make_float2(xe.x - tv.x, -(xe.y - tv.y));
-    };
-    float4* o = out + out_row * QROW;
-    for (int i = tid; i <= Q4; i += T) {
-        float2 x_i, x_bi, x_h, x_hb;
-        bins(i, x_i, x_bi);                          // X[i], X[B-i]
-        bins(B / 2 - i, x_h, x_hb);                  // X[B/2-i], X[B/2+i]
-        o[qa(i)] = make_float4(x_i.x, x_hb.x, x_i.y, x_hb.y);
-        o[qm(i)] = make_float4(x_bi.x, x_h.x, x_bi.y, x_h.y);
+        ifft_smem<14, C::R3, false>(buf, s_t2, s_a3, s_b3);   // buf = conj(Z)
+        // bins k and B-k from Z[k], Z[B-k]:  X[k] = Xe + conj(w^k)*Xo,  X[B-k] = conj(Xe - conj(w^k)*Xo)
+        auto bins = [&](int k, float2& xk, float2& xbk) {
+            const float2 zk = buf[pad(k)];
+            const float2 zp = buf[pad(k == 0 ? 0 : B - k)];
+            const float2 A = make_float2(zk.x, -zk.y), P = make_float2(zp.x, zp.y);     // Z[k], conj(Z[B-k])
+            const float2 xe = make_float2(0.5f * (A.x + P.x), 0.5f * (A.y + P.y));
+            const float2 dd = make_float2(A.x - P.x, A.y - P.y);
+            const float2 xo = make_float2(0.5f * dd.y, -0.5f * dd.x);                   // -i*dd/2
+            const float2 w = __ldg(tab.w + k);
+            const float2 tv = cmul(make_float2(w.x, -w.y), xo);
+            xk = make_float2(xe.x + tv.x, xe.y + tv.y);
+            xbk = make_float2(xe.x - tv.x, -(xe.y - tv.y));
+        };
+        float4* o = xout + out_row * QROW;
+        for (int i = tid; i <= Q4; i += T) {
+            float2 x_i, x_bi, x_h, x_hb;
+            bins(i, x_i, x_bi);                          // X[i], X[B-i]
+            bins(B / 2 - i, x_h, x_hb);                  // X[B/2-i], X[B/2+i]
+            o[qa(i)] = make_float4(x_i.x, x_hb.x, x_i.y, x_hb.y);
+            o[qm(i)] = make_float4(x_bi.x, x_h.x, x_bi.y, x_h.y);
+        }
+        __syncthreads();           // buf is the next row's
     }
 }
 
@@ -1360,9 +1382,10 @@ int launch_forward_quad_typed(const sb_stream* src, const QueryDesc* d_desc, int
         SB_CUDA(cudaFuncSetAttribute(k_forward_quad<S, MODE, MULTI>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem));
         attr_set = true;
     }
-    k_forward_quad<S, MODE, MULTI><<<(unsigned)rows, Cfg<14>::T, smem, c.stream>>>(
+    const int64_t grid = std::min<int64_t>(rows, c.sm_count);       // persistent: one CTA per SM walks the rows
+    k_forward_quad<S, MODE, MULTI><<<(unsigned)grid, Cfg<14>::T, smem, c.stream>>>(
         static_cast<const S*>(src->d_raw), src->n, src->d_pfx, d_desc, q_begin, q_end, row_first, tab,
-        reinterpret_cast<float4*>(out), MULTI ? m->d_streams : nullptr, MULTI ? m->d_slots : nullptr, row_list);
+        reinterpret_cast<float4*>(out), MULTI ? m->d_streams : nullptr, MULTI ? m->d_slots : nullptr, row_list, rows);
     SB_CUDA(cudaGetLastError());
     return SB_OK;
 }

@@ -31,13 +31,16 @@ __device__ constexpr float kS32[16] = {
     1.0f, 0.98078528040323043f, 0.92387953251128674f, 0.83146961230254524f,
     0.70710678118654752f, 0.55557023301960218f, 0.38268343236508978f, 0.19509032201612825f};
 
-// d * exp(+2*pi*i*q/32) with q a compile-time constant after unrolling
+// d * exp(+2*pi*i*q/32) with q a compile-time constant after unrolling.  The roundings are spelled out: with the
+// butterflies unrolled, a plain product would be free to fuse into the next stage's sum, and the spectra would
+// change in the last bit.
 __device__ __forceinline__ float2 rot32(float2 d, int q) {
     if (q == 0) return d;
     if (q == 8) return make_float2(-d.y, d.x);
-    if (q == 4) { const float h = 0.70710678118654752f; return make_float2((d.x - d.y) * h, (d.x + d.y) * h); }
-    if (q == 12) { const float h = 0.70710678118654752f; return make_float2(-(d.x + d.y) * h, (d.x - d.y) * h); }
-    return make_float2(d.x * kC32[q] - d.y * kS32[q], d.x * kS32[q] + d.y * kC32[q]);
+    const float h = 0.70710678118654752f;
+    if (q == 4) return make_float2(__fmul_rn(d.x - d.y, h), __fmul_rn(d.x + d.y, h));
+    if (q == 12) return make_float2(__fmul_rn(d.x + d.y, -h), __fmul_rn(d.x - d.y, h));
+    return make_float2(__fmaf_rn(d.x, kC32[q], -__fmul_rn(d.y, kS32[q])), __fmaf_rn(d.y, kC32[q], __fmul_rn(d.x, kS32[q])));
 }
 
 // In-register inverse DFT of R points (sign +, unnormalised), decimation in frequency: natural
@@ -51,21 +54,24 @@ template <int R> __device__ __forceinline__ constexpr int brev(int r) {
 // With KEEP < R only the outputs X[0 .. KEEP) are produced (KEEP >= R/2): position g of the
 // bit-reversed result holds X[brev(g)], so in the last stage the pair (g, g+1) holds X[r] and
 // X[r + R/2], r = brev(g), and the subtraction is skipped when r + R/2 >= KEEP.
+// Each stage is its own instantiation with a constant trip count: written as nested loops over h, g and a, the
+// compiler left the inner loops of the radix-32 and radix-16 passes rolled, with v[] in local memory and the
+// twiddles loaded from global memory in every butterfly.
+template <int R, int KEEP, int H>
+__device__ __forceinline__ void dft_dif_stage(float2 (&v)[R]) {
+#pragma unroll
+    for (int i = 0; i < R / 2; ++i) {
+        const int g = (i / H) * (2 * H), a = i % H;
+        const float2 x = v[g + a], y = v[g + a + H];
+        v[g + a] = cadd(x, y);
+        if (!(H == 1 && brev<R>(g) + R / 2 >= KEEP)) v[g + a + H] = rot32(csub(x, y), a * (16 / H));
+    }
+    if constexpr (H > 1) dft_dif_stage<R, KEEP, H / 2>(v);
+}
 template <int R, int KEEP = R>
 __device__ __forceinline__ void dft_dif(float2 (&v)[R]) {
     static_assert(KEEP >= R / 2 && KEEP <= R, "KEEP out of range");
-#pragma unroll
-    for (int h = R / 2; h >= 1; h >>= 1) {
-#pragma unroll
-        for (int g = 0; g < R; g += 2 * h) {
-#pragma unroll
-            for (int a = 0; a < h; ++a) {
-                const float2 x = v[g + a], y = v[g + a + h];
-                v[g + a] = cadd(x, y);
-                if (!(h == 1 && brev<R>(g) + R / 2 >= KEEP)) v[g + a + h] = rot32(csub(x, y), a * (16 / h));
-            }
-        }
-    }
+    dft_dif_stage<R, KEEP, R / 2>(v);
 }
 
 // one padding slot per 32 complex values keeps the radix-32 scatter of pass 1 conflict free
