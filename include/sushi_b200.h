@@ -39,7 +39,7 @@
 extern "C" {
 #endif
 
-#define SB_ABI_VERSION 2
+#define SB_ABI_VERSION 3
 
 /* status codes */
 #define SB_OK            0
@@ -53,6 +53,7 @@ extern "C" {
 #define SB_F32 1             /* 'float32'                                    */
 
 typedef struct sb_stream sb_stream;      /* opaque: one normalised stream in HBM */
+typedef struct sb_flac sb_flac;          /* opaque: an indexed FLAC file on the device */
 
 /* ---- life cycle ------------------------------------------------------- */
 
@@ -225,6 +226,25 @@ int sb_load_pcm(const void* pcm_host, int64_t frames, int channels, int sample_w
  * returned for the host mirror. */
 int sb_normalise(const sb_stream* raw_f32, int dtype, sb_stream** out,
                  float* min3_out, float* max3_out);
+
+/* ---- FLAC input (ABI version 3) -------------------------------------------
+ *
+ * A FLAC file loads exactly as the plain PCM WAV of its decoded samples loads through sb_load_pcm: 16-bit samples
+ * as they are, 24-bit ones by their top 16 bits.  Decoding runs on the GPU; the stream geometry stays with the
+ * caller, as it does for WAV, so indexing (which yields the sample count) and decoding are two calls.
+ *
+ * sb_flac_index uploads the whole file (`nbytes` bytes, metadata included; the caller has read STREAMINFO and
+ * passes its channel count, bits per sample and sample rate) and finds its frames: the first at
+ * first_frame_offset, each next one by its coded frame or sample number.  *frames_out receives the decoded samples
+ * per channel.  Only 16 and 24 bits per sample and 1 to 8 channels are accepted.
+ * sb_flac_decode decodes every frame, checks each frame's CRC-16 and that it ends exactly where the next frame
+ * (or the file) does, then resamples to sample_rate and pads exactly as sb_load_pcm does, into a SB_F32 stream for
+ * sb_normalise.  A corrupt file fails with SB_EINVAL and sb_last_error() names the frame and its byte offset;
+ * no samples are produced.  The STREAMINFO MD5 is not checked. */
+int sb_flac_index(const void* file, int64_t nbytes, int64_t first_frame_offset, int channels, int bits,
+                  int framerate, sb_flac** out, int64_t* frames_out);
+int sb_flac_decode(sb_flac* flac, int sample_rate, int64_t padding, int64_t total_len, sb_stream** out_f32);
+int sb_flac_destroy(sb_flac* flac);
 
 /* ---- multi-GPU: events shard across ranks (SURVEY.md 8e) ---------------- */
 

@@ -1,7 +1,8 @@
-"""The Sushi command line for WAV inputs: `python -m sushi_b200 --src a.wav --dst b.wav --script s.ass -o out.ass`.
+"""The Sushi command line for WAV and FLAC inputs: `python -m sushi_b200 --src a.wav --dst b.wav --script s.ass -o out.ass`.
 
 Flags, defaults and checks are the reference's (sushi.py:528-843).  Demuxing is not supported, so
---src and --dst must be WAV files; for those the reference starts no subprocess either.  Every
+--src and --dst must be WAV or FLAC files.  For a WAV file the reference starts no subprocess either; a FLAC file
+is decoded on the GPU, where the reference would have ffmpeg convert it (DESIGN.md section 2).  Every
 check runs before the GPU is touched; the run itself is pipeline.shift_script.
 """
 import argparse
@@ -68,7 +69,7 @@ def create_arg_parser():
     parser.add_argument('--sample-rate', default=12000, type=int, metavar='<rate>', dest='sample_rate',
                         help='Downsampled audio sample rate. [%(default)s]')
 
-    # stream indices select streams of a video; WAV inputs have one of each, so they are ignored
+    # stream indices select streams of a video; WAV and FLAC inputs have one of each, so they are ignored
     parser.add_argument('--src-audio', default=None, type=int, metavar='<id>', dest='src_audio_idx',
                         help='Audio stream index of the source video (ignored for WAV input)')
     parser.add_argument('--src-script', default=None, type=int, metavar='<id>', dest='src_script_idx',
@@ -99,9 +100,9 @@ def create_arg_parser():
                         help='Timecodes file to use instead of making one from the source (when possible)')
 
     parser.add_argument('--src', required=True, dest='source', metavar='<filename>',
-                        help='Source audio (WAV)')
+                        help='Source audio (WAV or FLAC)')
     parser.add_argument('--dst', required=True, dest='destination', metavar='<filename>',
-                        help='Destination audio (WAV)')
+                        help='Destination audio (WAV or FLAC)')
     parser.add_argument('-o', '--output', default=None, dest='output_script', metavar='<filename>',
                         help='Output script')
 
@@ -112,12 +113,12 @@ def create_arg_parser():
 
 
 def _require_wav(path):
-    if get_extension(path) != '.wav':
-        raise SushiError('{0}: demuxing is not supported, convert the input to WAV first'.format(path))
+    if get_extension(path) not in ('.wav', '.flac'):
+        raise SushiError('{0}: demuxing is not supported, convert the input to WAV or FLAC first'.format(path))
 
 
 def run(args):
-    """sushi.py:528-736 for WAV inputs.  Everything up to the shift_script call is validation and
+    """sushi.py:528-736 for WAV and FLAC inputs.  Everything up to the shift_script call is validation and
     small text files; nothing before it touches the GPU."""
     ignore_chapters = args.chapters_file is not None and args.chapters_file.lower() == 'none'
 

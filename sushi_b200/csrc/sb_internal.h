@@ -144,6 +144,10 @@ int launch_part_spectra(const sb_stream* tmpl, int hd, const QueryDesc* d_desc, 
                         int64_t part_first, int64_t rows, float2* out);
 void fused_release_tables();
 
+// sb_loader.cu: sb_load_pcm after its host-to-device copy (the FLAC decoder feeds it decoded int16 PCM on the device)
+int load_pcm_device(const unsigned char* d_pcm, int64_t frames, int channels, int sample_width, int framerate,
+                    int sample_rate, int64_t padding, int64_t total_len, sb_stream** out_f32, const char* who);
+
 int get_plan(int type, int64_t batch, cufftHandle* out);
 void drop_plans();
 

@@ -294,19 +294,13 @@ int medians_from_histograms(const sb_stream* raw, float* med_pos, float* med_neg
 
 int py2_round_pos(double x) { return (int)floor(x + 0.5); }     // round() of Python 2 for x >= 0 (wav.py:127)
 
-}  // namespace
-
-extern "C" {
-
-int sb_load_pcm(const void* pcm_host, int64_t frames, int channels, int sample_width,
-                int framerate, int sample_rate, int64_t padding, int64_t total_len,
-                sb_stream** out_f32) {
-    Ctx& c = ctx();
-    if (!c.inited) SB_FAIL(SB_ESTATE, "sb_load_pcm: library not initialised (call sb_init)");
-    if (!pcm_host || !out_f32) SB_FAIL(SB_EINVAL, "sb_load_pcm: NULL argument");
+// The geometry of one load: the chunk loop of the reference (wav.py:113-137) over `frames` frames, and the kernel's
+// work items.  Checks the arguments; `who` prefixes the messages.
+int plan_load(int64_t frames, int channels, int sample_width, int framerate, int sample_rate, int64_t padding,
+              int64_t total_len, const char* who, ResampleGeom* gout, LoadItems* liout) {
     if (sample_width != 2 && sample_width != 3) SB_FAIL(SB_EINVAL, "Unsupported sample width: %d", sample_width);
     if (frames < 0 || channels < 1 || framerate < 1 || sample_rate < 1 || padding < 0 || total_len < 1)
-        SB_FAIL(SB_EINVAL, "sb_load_pcm: bad geometry");
+        SB_FAIL(SB_EINVAL, "%s: bad geometry", who);
     ResampleGeom g;
     g.frames = frames; g.framerate = framerate;
     g.nfull = frames / framerate;
@@ -324,35 +318,71 @@ int sb_load_pcm(const void* pcm_host, int64_t frames, int channels, int sample_w
     // file).  Samples past the content region are overwritten by the tail padding there and are not written here;
     // samples past the end of the buffer make the reference's copy fail.
     if (g.written > total_len - padding)
-        SB_FAIL(SB_EINVAL, "sb_load_pcm: %lld resampled samples run past a buffer of %lld with %lld padding",
-                (long long)g.written, (long long)total_len, (long long)padding);
-
-    if (channels > kMaxChannels) SB_FAIL(SB_EINVAL, "sb_load_pcm: %d channels (at most %d)", channels, kMaxChannels);
-    sb_stream* s = new (std::nothrow) sb_stream();
-    if (!s) SB_FAIL(SB_ENOMEM, "sb_load_pcm: out of host memory");
-    s->n = total_len; s->dtype = SB_F32; s->pcm_channels = channels;
-    unsigned char* d_pcm = nullptr;
-    const size_t pcm_bytes = (size_t)frames * channels * sample_width;
-    int rc = pool_alloc(&s->d_raw, sizeof(float) * total_len + 16);
-    if (rc == SB_OK) rc = pool_alloc((void**)&d_pcm, pcm_bytes + 16);
-    if (rc == SB_OK) rc = pool_alloc((void**)&s->d_loadhist, sizeof(unsigned long long) * (kCoarseBins + 1));
-    if (rc != SB_OK) { pool_free(s->d_raw); pool_free(d_pcm); delete s; return rc; }
+        SB_FAIL(SB_EINVAL, "%s: %lld resampled samples run past a buffer of %lld with %lld padding",
+                who, (long long)g.written, (long long)total_len, (long long)padding);
+    if (channels > kMaxChannels) SB_FAIL(SB_EINVAL, "%s: %d channels (at most %d)", who, channels, kMaxChannels);
     LoadItems li;
     li.per_full = (g.out_full + 1023) / 1024; li.per_last = (g.out_last + 1023) / 1024;
     li.n_content = g.nfull * (int64_t)li.per_full + li.per_last;
     li.n_head = (padding + 1023) / 1024; li.n_tail = (padding + 1023) / 1024;
-    cudaError_t e = cudaMemcpyAsync(d_pcm, pcm_host, pcm_bytes, cudaMemcpyHostToDevice, c.stream);
-    if (e == cudaSuccess) e = cudaMemsetAsync(s->d_loadhist, 0, sizeof(unsigned long long) * (kCoarseBins + 1), c.stream);
+    *gout = g; *liout = li;
+    return SB_OK;
+}
+
+}  // namespace
+
+namespace sb {
+
+// Everything of sb_load_pcm after the PCM is on the device: allocate the float32 stream and its coarse histogram and
+// enqueue k_decode_resample_pad on the library stream.  d_pcm must stay valid until that work has run.
+int load_pcm_device(const unsigned char* d_pcm, int64_t frames, int channels, int sample_width, int framerate,
+                    int sample_rate, int64_t padding, int64_t total_len, sb_stream** out_f32, const char* who) {
+    Ctx& c = ctx();
+    ResampleGeom g; LoadItems li;
+    SB_TRY(plan_load(frames, channels, sample_width, framerate, sample_rate, padding, total_len, who, &g, &li));
+    sb_stream* s = new (std::nothrow) sb_stream();
+    if (!s) SB_FAIL(SB_ENOMEM, "%s: out of host memory", who);
+    s->n = total_len; s->dtype = SB_F32; s->pcm_channels = channels;
+    int rc = pool_alloc(&s->d_raw, sizeof(float) * total_len + 16);
+    if (rc == SB_OK) rc = pool_alloc((void**)&s->d_loadhist, sizeof(unsigned long long) * (kCoarseBins + 1));
+    if (rc != SB_OK) { pool_free(s->d_raw); delete s; return rc; }
+    cudaError_t e = cudaMemsetAsync(s->d_loadhist, 0, sizeof(unsigned long long) * (kCoarseBins + 1), c.stream);
     if (e == cudaSuccess) {
         ProfScope ps("decode_resample_pad");
         k_decode_resample_pad<<<c.sm_count * 8, 256, 0, c.stream>>>(
             d_pcm, g, li, channels, sample_width, static_cast<float*>(s->d_raw), s->d_loadhist);
         e = cudaGetLastError();
     }
-    if (e == cudaSuccess) e = cudaStreamSynchronize(c.stream);            // pcm_host may be reused by the caller
-    pool_free(d_pcm);
-    if (e != cudaSuccess) { sb_stream_destroy(s); SB_FAIL(SB_ECUDA, "sb_load_pcm: %s", cudaGetErrorString(e)); }
+    if (e != cudaSuccess) { sb_stream_destroy(s); SB_FAIL(SB_ECUDA, "%s: %s", who, cudaGetErrorString(e)); }
     *out_f32 = s;                 // no running sums yet: only sb_normalise / sb_stream_read accept it
+    return SB_OK;
+}
+
+}  // namespace sb
+
+extern "C" {
+
+int sb_load_pcm(const void* pcm_host, int64_t frames, int channels, int sample_width,
+                int framerate, int sample_rate, int64_t padding, int64_t total_len,
+                sb_stream** out_f32) {
+    Ctx& c = ctx();
+    if (!c.inited) SB_FAIL(SB_ESTATE, "sb_load_pcm: library not initialised (call sb_init)");
+    if (!pcm_host || !out_f32) SB_FAIL(SB_EINVAL, "sb_load_pcm: NULL argument");
+    ResampleGeom g; LoadItems li;
+    SB_TRY(plan_load(frames, channels, sample_width, framerate, sample_rate, padding, total_len, "sb_load_pcm", &g, &li));
+    unsigned char* d_pcm = nullptr;
+    const size_t pcm_bytes = (size_t)frames * channels * sample_width;
+    SB_TRY(pool_alloc((void**)&d_pcm, pcm_bytes + 16));
+    sb_stream* s = nullptr;
+    cudaError_t e = cudaMemcpyAsync(d_pcm, pcm_host, pcm_bytes, cudaMemcpyHostToDevice, c.stream);
+    if (e != cudaSuccess) { pool_free(d_pcm); SB_FAIL(SB_ECUDA, "sb_load_pcm: %s", cudaGetErrorString(e)); }
+    const int rc = load_pcm_device(d_pcm, frames, channels, sample_width, framerate, sample_rate, padding, total_len, &s,
+                                   "sb_load_pcm");
+    e = cudaStreamSynchronize(c.stream);                                  // pcm_host may be reused by the caller
+    pool_free(d_pcm);
+    if (rc != SB_OK) return rc;
+    if (e != cudaSuccess) { sb_stream_destroy(s); SB_FAIL(SB_ECUDA, "sb_load_pcm: %s", cudaGetErrorString(e)); }
+    *out_f32 = s;
     return SB_OK;
 }
 

@@ -95,7 +95,7 @@ def _resolve_links(events):
 
 def shift_script(src_audio, dst_audio, script_path, output_path, sample_rate=12000, sample_type='uint8',
                  chapter_times=(), **options):
-    """src/dst WAV + ASS/SRT script in, shifted script out (the WAV-in/script-out core of the CLI).
+    """src/dst WAV or FLAC + ASS/SRT script in, shifted script out (the audio-in/script-out core of the CLI).
     `options` are shift_events' keyword arguments, keyframes included."""
     script = load_script(script_path)
     script.sort_by_time()

@@ -110,6 +110,84 @@ class DownmixedWavFile(object):
         return decode_downmix(self.read_raw(count), self.sample_width, self.channels_count)
 
 
+FLAC_MAGIC = b'fLaC'
+FLAC_BLOCK_NAMES = {0: 'STREAMINFO', 1: 'PADDING', 2: 'APPLICATION', 3: 'SEEKTABLE', 4: 'VORBIS_COMMENT', 5: 'CUESHEET',
+                    6: 'PICTURE'}
+
+
+def id3v2_size(head):
+    """Bytes of an ID3v2 tag at the start of `head` (header, syncsafe size, optional footer), or 0 if there is none."""
+    if len(head) < 10 or head[0:3] != b'ID3':
+        return 0
+    size = (head[6] & 0x7F) << 21 | (head[7] & 0x7F) << 14 | (head[8] & 0x7F) << 7 | (head[9] & 0x7F)
+    return 10 + size + (10 if head[5] & 0x10 else 0)
+
+
+def is_flac(path):
+    """True when the file starts with the FLAC marker, or with an ID3v2 tag and then the marker (False when it cannot
+    be read: the WAV reader reports that)."""
+    try:
+        f = open(path, 'rb')
+    except OSError:
+        return False
+    with f:
+        head = f.read(10)
+        if head[0:4] == FLAC_MAGIC:
+            return True
+        skip = id3v2_size(head)
+        if not skip:
+            return False
+        f.seek(skip)
+        return f.read(4) == FLAC_MAGIC
+
+
+class FlacFile(object):
+    """FLAC metadata reader: an optional leading ID3v2 tag, the marker, then the metadata blocks.  STREAMINFO (which
+    must come first) gives the stream parameters; every other block (PADDING, APPLICATION, SEEKTABLE, VORBIS_COMMENT,
+    CUESHEET, PICTURE) is skipped.  `frame_offset` is where the first audio frame starts; the frames are decoded on the
+    GPU (sb_flac_index / sb_flac_decode)."""
+
+    def __init__(self, path):
+        with open(path, 'rb') as f:
+            self.data = f.read()
+        d = self.data
+        at = id3v2_size(d[:10])
+        if d[at:at + 4] != FLAC_MAGIC:
+            raise SushiError('{0}: not a FLAC file'.format(path))
+        at += 4
+        self.blocks = []
+        have_info = False
+        while True:
+            if at + 4 > len(d):
+                raise SushiError('{0}: FLAC metadata block header at byte {1} is truncated'.format(path, at))
+            last, kind = d[at] >> 7, d[at] & 0x7F
+            size = int.from_bytes(d[at + 1:at + 4], 'big')
+            body = d[at + 4:at + 4 + size]
+            if len(body) < size or kind == 127:
+                raise SushiError('{0}: invalid FLAC metadata block at byte {1}'.format(path, at))
+            if (kind == 0) != (not self.blocks):
+                raise SushiError('{0}: STREAMINFO must be the first and only STREAMINFO metadata block'.format(path))
+            if kind == 0:
+                if size < 34:
+                    raise SushiError('{0}: STREAMINFO of {1} bytes'.format(path, size))
+                self.min_block, self.max_block = struct.unpack('>HH', body[0:4])
+                packed = int.from_bytes(body[10:18], 'big')
+                self.framerate = packed >> 44
+                self.channels_count = ((packed >> 41) & 7) + 1
+                self.bits_per_sample = ((packed >> 36) & 31) + 1
+                self.total_samples = packed & ((1 << 36) - 1)
+                have_info = True
+            self.blocks.append(FLAC_BLOCK_NAMES.get(kind, 'reserved {0}'.format(kind)))
+            at += 4 + size
+            if last:
+                break
+        if not have_info:
+            raise SushiError('{0}: FLAC file without STREAMINFO'.format(path))
+        if self.framerate < 1:
+            raise SushiError('{0}: FLAC STREAMINFO sample rate is 0'.format(path))
+        self.frame_offset = at
+
+
 def decode_downmix(raw, sample_width, channels):
     """bytes -> float32 mono; int24 keeps the top 16 bits (wav.py:68-74); channels are
     summed left to right in float32, then divided (wav.py:88-90)."""
@@ -230,6 +308,10 @@ class WavStream(StreamGeometry):
             raise SushiError('Unknown sample type of WAV stream, must be uint8 or float32')
         self._handle = None
         before_read = time()
+        if is_flac(path):
+            self._load_flac(path, sample_rate, sample_type, device, loader)
+            logging.info('Done reading FLAC {0} in {1}s'.format(path, time() - before_read))
+            return
         stream = DownmixedWavFile(path)
         try:
             if loader == 'gpu':
@@ -250,6 +332,38 @@ class WavStream(StreamGeometry):
             stream.close()
         logging.info('Done reading WAV {0} in {1}s'.format(path, time() - before_read))
 
+    def _load_flac(self, path, sample_rate, sample_type, device, loader):
+        """A FLAC file loads exactly as the plain PCM WAV of its decoded samples: the frames are decoded on the GPU
+        into the int16 PCM sb_load_pcm would read from that WAV (24-bit samples keep their top 16 bits), and the
+        rest is the WAV path.  There is no host decoder, so loader='host' is refused."""
+        flac = FlacFile(path)
+        if flac.bits_per_sample not in (16, 24):
+            raise SushiError('FLAC with {0} bits per sample is not supported (16 or 24)'.format(flac.bits_per_sample))
+        if loader != 'gpu':
+            raise SushiError("{0}: FLAC input needs loader='gpu' (there is no host FLAC decoder)".format(path))
+        lib = _native.lib(device)
+        h = ctypes.c_void_p()
+        frames = ctypes.c_int64()
+        buf = np.frombuffer(flac.data, dtype=np.uint8)
+        with nvtx_range('sushi_b200: sb_flac_index'):
+            _native.check(lib.sb_flac_index(buf.ctypes.data_as(ctypes.c_void_p), len(flac.data), flac.frame_offset,
+                                            flac.channels_count, flac.bits_per_sample, flac.framerate,
+                                            ctypes.byref(h), ctypes.byref(frames)), 'sb_flac_index')
+        try:
+            def decode(padding, total):
+                raw = ctypes.c_void_p()
+                with nvtx_range('sushi_b200: sb_flac_decode'):
+                    _native.check(lib.sb_flac_decode(h, sample_rate, padding, total, ctypes.byref(raw)), 'sb_flac_decode')
+                # after the frames passed their checks, which name a damaged frame more precisely than the total does
+                if flac.total_samples and flac.total_samples != frames.value:
+                    lib.sb_stream_destroy(raw)
+                    raise SushiError('{0}: FLAC STREAMINFO says {1} samples, the frames hold {2}'.format(
+                        path, flac.total_samples, frames.value))
+                return raw
+            self._load_gpu_with(decode, frames.value, flac.framerate, sample_rate, sample_type, device)
+        finally:
+            lib.sb_flac_destroy(h)
+
     def _load_gpu(self, pcm, frames, channels, sample_width, framerate, sample_rate, sample_type, device):
         """wav.py:108-156 on the GPU: geometry here (same scalar code as the reference), arithmetic
         in sb_load_pcm / sb_normalise; .data is then mirrored back for get_substream views.  `frames` is the
@@ -258,6 +372,20 @@ class WavStream(StreamGeometry):
         if sample_width not in (2, 3):
             raise SushiError('Unsupported sample width: {0}'.format(sample_width))
         decoded = len(pcm) // (channels * sample_width)
+        buf = np.frombuffer(pcm, dtype=np.uint8, count=decoded * channels * sample_width)
+
+        def load(padding, total):
+            raw = ctypes.c_void_p()
+            with nvtx_range('sushi_b200: sb_load_pcm'):
+                _native.check(lib.sb_load_pcm(buf.ctypes.data_as(ctypes.c_void_p), decoded, channels, sample_width,
+                                              framerate, sample_rate, padding, total, ctypes.byref(raw)), 'sb_load_pcm')
+            return raw
+        lib = _native.lib(device)
+        self._load_gpu_with(load, frames, framerate, sample_rate, sample_type, device)
+
+    def _load_gpu_with(self, load, frames, framerate, sample_rate, sample_type, device):
+        """The geometry of wav.py:113-120 for `frames` frames at `framerate`, then load(padding, total) -> the raw
+        float32 stream (sb_load_pcm or sb_flac_decode), normalised by sb_normalise and mirrored back."""
         total_seconds = frames / float(framerate)
         self.sample_count = math.ceil(total_seconds * sample_rate)
         self.sample_rate = sample_rate
@@ -265,11 +393,7 @@ class WavStream(StreamGeometry):
         self.padding_size = 10 * framerate
         total = int(self.PADDING_SECONDS * 2 * framerate + self.sample_count)
         lib = _native.lib(device)
-        raw = ctypes.c_void_p()
-        buf = np.frombuffer(pcm, dtype=np.uint8, count=decoded * channels * sample_width)
-        with nvtx_range('sushi_b200: sb_load_pcm'):
-            _native.check(lib.sb_load_pcm(buf.ctypes.data_as(ctypes.c_void_p), decoded, channels, sample_width,
-                                          framerate, sample_rate, self.padding_size, total, ctypes.byref(raw)), 'sb_load_pcm')
+        raw = load(self.padding_size, total)
         h = ctypes.c_void_p()
         lo, hi = ctypes.c_float(), ctypes.c_float()
         try:
