@@ -39,12 +39,12 @@
 extern "C" {
 #endif
 
-#define SB_ABI_VERSION 3
+#define SB_ABI_VERSION 4
 
 /* status codes */
 #define SB_OK            0
 #define SB_EINVAL       -1   /* bad argument (range, NULL, dtype)            */
-#define SB_ECUDA        -2   /* CUDA runtime / cuFFT failure                 */
+#define SB_ECUDA        -2   /* CUDA runtime failure                         */
 #define SB_ENOMEM       -3   /* host or device allocation failed             */
 #define SB_ESTATE       -4   /* library not initialised / already shut down  */
 
@@ -58,7 +58,7 @@ typedef struct sb_flac sb_flac;          /* opaque: an indexed FLAC file on the 
 /* ---- life cycle ------------------------------------------------------- */
 
 /* Bind the calling process to CUDA device `device` and create the library
- * stream, plans and scratch.  Idempotent for the same device. */
+ * stream and scratch.  Idempotent for the same device. */
 int sb_init(int device);
 int sb_shutdown(void);
 /* ABI version of the loaded library (compare with SB_ABI_VERSION). */
@@ -67,32 +67,32 @@ int sb_abi_version(void);
 const char* sb_last_error(void);
 /* Wait until everything enqueued on the library stream has finished. */
 int sb_sync(void);
-/* Tuning knobs (power-of-two lag-block size in samples, 1024..65536; items per
- * chunk).  Changing the block size drops cached block spectra. */
+/* Lag-block size in samples.  Every engine runs at 16384 (the FFT size is twice that); sb_set_block_size
+ * accepts 16384 and fails with SB_EINVAL for anything else. */
 int sb_set_block_size(int block);
 int sb_get_block_size(void);
 /* Engine behind sb_find*:
  *   2 (default) = the packed fused lag-block kernels (sb_fused2.cu): spectral multiply, inverse FFT in
  *       shared memory, normalisation and argmin in one launch, on spectra stored in a paired layout;
- *       lag blocks of 16384 at hop B -- any other geometry silently runs engine 1, and templates of 12+
- *       partitions keep engine 1's blocked multiply.  One CTA handles one lag block, or (batches averaging
- *       >= 4 template partitions) a pair of consecutive lag blocks that share their template rows, the
- *       second product spectrum waiting in an L2-resident scratch; both give bit-identical results;
+ *       templates of 12+ partitions keep engine 1's blocked multiply.  One CTA handles one lag block, or
+ *       (batches averaging >= 4 template partitions) a pair of consecutive lag blocks that share their
+ *       template rows, the second product spectrum waiting in an L2-resident scratch; both give
+ *       bit-identical results;
  *   4 / 5 = engine 2 with pairs always / never;
- *   1 = the first fused lag-block kernel (sb_fused.cu; lag blocks of 8192 or 16384, hop B or B/2);
- *   0 = the cuFFT-planned pipeline (any block size; kept as the cross-check and for odd block sizes).
- * Engines agree to float32 FFT rounding (~2e-7 of the curve), not bit for bit. */
+ *   1 = the first fused lag-block kernel (sb_fused.cu).
+ * Any other value fails with SB_EINVAL.  Engines agree to float32 FFT rounding (~2e-7 of the curve), not
+ * bit for bit. */
 int sb_set_engine(int engine);
 int sb_get_engine(void);
-/* Spectral multiply of engine 1: 0 (default) = per lag block inside the fused kernel, except for
- * queries whose template spans 12 or more partitions (>= 16 s at the default block size), which go
- * through the register-blocked multiply kernel (8 lag blocks share each template row); 1 = never
- * blocked, 2 = always blocked.  The route depends only on the query, not on the rest of the batch. */
+/* Spectral multiply, every engine: 0 (default) = per lag block inside the fused kernel, except for
+ * queries whose template spans 12 or more partitions (>= 16.4 s at 12 kHz), which go through the
+ * register-blocked multiply kernel (8 lag blocks share each template row) and engine 1's fused kernel;
+ * 1 = never blocked, 2 = always blocked.  The route depends only on the query, not on the rest of the
+ * batch. */
 int sb_set_premac_mode(int mode);
-/* Overlap-save geometry of the fused engines: 1 (default) = hop B (half of each inverse FFT is valid
- * lags), 2 = hop B/2 (three quarters valid, but twice as many template partitions to multiply:
- * pays off only for templates shorter than B/2), 0 = chosen per batch by a cost rule.  Geometries
- * agree to float32 FFT rounding (~1e-7), not bit for bit, so a run should stick to one. */
+/* Overlap-save geometry: every engine runs at hop B (template partitions of B samples, half of each
+ * inverse FFT is valid lags).  sb_set_hop_mode accepts 1 (hop B) and fails with SB_EINVAL for anything
+ * else. */
 int sb_set_hop_mode(int mode);
 /* Body variant of the packed kernels (engines 2, 4, 5) on uint8 streams: 3 (default) = per run of 8 lags a lower
  * and an upper bound of the screening values from the run's largest correlation value and its exact head sums; only
@@ -106,8 +106,6 @@ int sb_set_hop_mode(int mode);
  * dropped in round 2.) */
 int sb_set_epilogue(int variant);
 int sb_get_epilogue(void);
-/* Lag blocks processed per multiply / inverse-FFT / normalise launch (>= 1). */
-int sb_set_chunk_items(int items);
 /* Template partition spectra kept resident per pass over a batch (>= 1); batches needing more are
  * processed in several passes of whole queries. */
 int sb_set_max_parts(int64_t parts);
@@ -189,9 +187,9 @@ int sb_match_curves(const sb_stream* image, const sb_stream* tmpl, int64_t count
  * against the query's own streams.  All streams must share one sample type and carry running sums; a NULL entry,
  * a slot outside [0, n_streams), a stream without running sums or mixed sample types fail with SB_EINVAL, and
  * sb_last_error() names the query or slot.
- * The packed engine (2, 4, 5 at the default geometry) runs the whole call in one set of launches whatever the number
- * of streams; queries of the blocked class (templates of 12+ partitions) and other engines / geometries run as one
- * sb_find_batch-like pass per distinct (image, template) pair inside the call. */
+ * The packed engine (2, 4, 5) runs the whole call in one set of launches whatever the number of streams; queries of
+ * the blocked class (templates of 12+ partitions) and engine 1 run as one sb_find_batch-like pass per distinct
+ * (image, template) pair inside the call. */
 int sb_find_multi(const sb_stream* const* streams, int32_t n_streams, int64_t count,
                   const int32_t* image_slot, const int32_t* tmpl_slot,
                   const int64_t* tmpl_off, const int64_t* tmpl_len,

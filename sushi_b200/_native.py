@@ -14,7 +14,7 @@ LIB_PATH = os.path.join(_HERE, 'libsushi_b200.so')
 
 SB_OK = 0
 SB_U8, SB_F32 = 0, 1
-ABI_VERSION = 3
+ABI_VERSION = 4
 
 c_i64 = ctypes.c_int64
 c_i64p = ctypes.POINTER(ctypes.c_int64)
@@ -31,7 +31,6 @@ PROTOTYPES = {
     'sb_sync': (ctypes.c_int, []),
     'sb_set_block_size': (ctypes.c_int, [ctypes.c_int]),
     'sb_get_block_size': (ctypes.c_int, []),
-    'sb_set_chunk_items': (ctypes.c_int, [ctypes.c_int]),
     'sb_set_engine': (ctypes.c_int, [ctypes.c_int]),
     'sb_set_max_parts': (ctypes.c_int, [c_i64]),
     'sb_get_engine': (ctypes.c_int, []),

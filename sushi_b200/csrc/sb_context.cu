@@ -1,4 +1,4 @@
-// Library context: device binding, error text, cuFFT plan cache, timers and the
+// Library context: device binding, error text, device memory pool, timers and the
 // per-kernel-class accounting used by bench.py's roofline block.
 #include "sb_internal.h"
 #include <cstdarg>
@@ -105,34 +105,6 @@ void pool_release_all() {
     g_free_blocks.clear(); g_cached_bytes = 0;
 }
 
-int get_plan(int type, int64_t batch, cufftHandle* out) {
-    Ctx& c = ctx();
-    auto key = std::make_pair(type, batch);
-    auto it = c.plans.find(key);
-    if (it != c.plans.end()) { *out = it->second; return SB_OK; }
-    if (c.plans.size() >= 24) drop_plans();
-    cufftHandle h;
-    int n[1] = {2 * c.B};
-    int real_embed[1] = {2 * c.B + 2};
-    int cplx_embed[1] = {c.B + 1};
-    // in-place layouts: a row is (B+1) complex = (2B+2) floats
-    if (type == CUFFT_R2C) {
-        SB_CUFFT(cufftPlanMany(&h, 1, n, real_embed, 1, 2 * c.B + 2, cplx_embed, 1, c.B + 1, CUFFT_R2C, (int)batch));
-    } else {
-        SB_CUFFT(cufftPlanMany(&h, 1, n, cplx_embed, 1, c.B + 1, real_embed, 1, 2 * c.B + 2, CUFFT_C2R, (int)batch));
-    }
-    SB_CUFFT(cufftSetStream(h, c.stream));
-    c.plans[key] = h;
-    *out = h;
-    return SB_OK;
-}
-
-void drop_plans() {
-    Ctx& c = ctx();
-    for (auto& kv : c.plans) cufftDestroy(kv.second);
-    c.plans.clear();
-}
-
 }  // namespace sb
 
 using namespace sb;
@@ -176,7 +148,6 @@ int sb_shutdown(void) {
     if (!c.inited) return SB_OK;
     cudaStreamSynchronize(c.stream);
     prof_collect();
-    drop_plans();
     pool_release_all();
     fused_release_tables();
     packed_release_tables();
@@ -198,22 +169,12 @@ int sb_sync(void) {
 }
 
 int sb_set_block_size(int block) {
-    Ctx& c = ctx();
-    if (block < 1024 || block > 65536 || (block & (block - 1)))
-        SB_FAIL(SB_EINVAL, "sb_set_block_size: %d is not a power of two in [1024, 65536]", block);
-    if (block == c.B) return SB_OK;
-    if (c.inited) { cudaStreamSynchronize(c.stream); drop_plans(); }
-    c.B = block;
-    // scratch is sized in rows of (B+1) complex: force re-allocation
-    if (c.inited) {
-        cudaFree(c.d_parts); c.d_parts = nullptr; c.parts_cap = 0;
-        cudaFree(c.d_items); c.d_items = nullptr; c.items_cap = 0;
-    }
+    if (block != kLagBlock) SB_FAIL(SB_EINVAL, "sb_set_block_size: %d is not %d, the only lag-block size", block, kLagBlock);
     return SB_OK;
 }
-int sb_get_block_size(void) { return ctx().B; }
+int sb_get_block_size(void) { return kLagBlock; }
 int sb_set_engine(int engine) {
-    if (engine < 0 || engine > 5 || engine == 3) SB_FAIL(SB_EINVAL, "sb_set_engine: %d is not one of 0 (cuFFT pipeline), 1 (fused kernel), 2 (packed fused kernels), 4 / 5 (packed kernel always / never over pairs of lag blocks)", engine);
+    if (engine < 1 || engine > 5 || engine == 3) SB_FAIL(SB_EINVAL, "sb_set_engine: %d is not one of 1 (fused kernel), 2 (packed fused kernels), 4 / 5 (packed kernel always / never over pairs of lag blocks)", engine);
     ctx().engine = engine;
     return SB_OK;
 }
@@ -224,8 +185,7 @@ int sb_set_premac_mode(int mode) {
     return SB_OK;
 }
 int sb_set_hop_mode(int mode) {
-    if (mode < 0 || mode > 2) SB_FAIL(SB_EINVAL, "sb_set_hop_mode: %d is not 0 (auto), 1 (hop B) or 2 (hop B/2)", mode);
-    ctx().hop_mode = mode;
+    if (mode != 1) SB_FAIL(SB_EINVAL, "sb_set_hop_mode: %d is not 1 (hop B), the only overlap-save geometry", mode);
     return SB_OK;
 }
 int sb_set_epilogue(int variant) {
@@ -237,11 +197,6 @@ int sb_get_epilogue(void) { return ctx().epilogue; }
 int sb_set_max_parts(int64_t parts) {
     if (parts < 1) SB_FAIL(SB_EINVAL, "sb_set_max_parts: %lld < 1", (long long)parts);
     ctx().max_parts = parts;
-    return SB_OK;
-}
-int sb_set_chunk_items(int items) {
-    if (items < 1 || items > (1 << 20)) SB_FAIL(SB_EINVAL, "sb_set_chunk_items: %d out of range", items);
-    ctx().chunk_items = items;
     return SB_OK;
 }
 

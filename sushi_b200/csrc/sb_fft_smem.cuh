@@ -1,17 +1,15 @@
 // Shared-memory FFT machinery of the fused engines: geometry, twiddle tables and the in-place
-// Stockham inverse transform (used by sb_fused.cu and, for the forward spectra, sb_fused2.cu).
+// Stockham inverse transform of N = B = 16384 complex points (used by sb_fused.cu and, for the
+// forward spectra, sb_fused2.cu).
 #pragma once
 #include "sb_fused_common.cuh"
 
 namespace sbf {
 
 // ---------------------------------------------------------------- configuration
-template <int LOGN> struct Cfg;
+template <int LOG2N> struct Cfg;
 template <> struct Cfg<14> {   // B = 16384 lags per item
     static constexpr int N = 16384, T = 512, R1 = 32, R2 = 32, R3 = 16, MINB = 1;
-};
-template <> struct Cfg<13> {   // B = 8192 lags per item
-    static constexpr int N = 8192, T = 256, R1 = 32, R2 = 16, R3 = 16, MINB = 2;
 };
 
 struct FusedTables {
@@ -27,10 +25,10 @@ struct FusedTables {
 // k = j mod Ns, and writes out[(j-k)*R + k + r*Ns]; every value sits in a register between the two
 // barriers of a pass, so the transform is in place and the output is in natural order.
 // Must be entered after a barrier that made buf visible; ends with a barrier.
-template <int LOGN, int KEEP3, bool FUSED>
+template <int KEEP3, bool FUSED>
 __device__ __forceinline__ void ifft_smem(float2* __restrict__ buf, const float2* __restrict__ s_t2,
                                           const float2* __restrict__ s_a3, const float2* __restrict__ s_b3) {
-    typedef Cfg<LOGN> C;
+    typedef Cfg<14> C;
     constexpr int N = C::N, T = C::T;
     const int tid = threadIdx.x, lane = tid & 31;
     // Stockham passes: butterfly j reads in[j + r*N/R], twiddles by exp(2*pi*i*r*k/(Ns*R)),
@@ -104,6 +102,6 @@ __device__ __forceinline__ void ifft_smem(float2* __restrict__ buf, const float2
 }  // namespace sbf
 
 namespace sb {
-// device-resident twiddle tables for FFT half-size 2^logn (13 or 14); built on first use
-int fused_tables(int logn, sbf::FusedTables* out);
+// device-resident twiddle tables of Cfg<14>; built on first use
+int fused_tables(sbf::FusedTables* out);
 }

@@ -5,9 +5,8 @@
 //   4. slides the window sums through its lags, screens every lag in fp32 and evaluates only the
 //      lags that can still be the minimum with OpenCV's rule in fp64, and
 //   5. merges its (value, first index) into the query's result with one 64-bit atomicMin.
-// The B-long correlation block never touches HBM (the cuFFT pipeline in sb_matcher.cu writes and
-// re-reads it twice); the only global traffic is the spectra (L2 resident) and 2 B per lag of raw
-// samples.  See DESIGN.md section 4 for the roofline of each phase.
+// The B-long correlation block never touches HBM; the only global traffic is the spectra (L2
+// resident) and 2 B per lag of raw samples.  See DESIGN.md section 4 for the roofline of each phase.
 #include "sb_internal.h"
 #include <cmath>
 #include <cstdlib>
@@ -21,23 +20,25 @@ using namespace sbf;
 
 namespace {
 
+typedef Cfg<14> C;
+static_assert(C::N == kLagBlock, "the FFT half-size is the lag block");
+
 // ---------------------------------------------------------------- the kernel
-template <int LOGN, typename S, int HD>
-__global__ void __launch_bounds__(Cfg<LOGN>::T, Cfg<LOGN>::MINB)
+template <typename S>
+__global__ void __launch_bounds__(C::T, C::MINB)
 k_match_fused(const float2* __restrict__ That, int64_t part_first, const float2* __restrict__ Ypre,
               const float2* __restrict__ Xhat, int64_t nblk,
               const S* __restrict__ img, int64_t img_n,
               const double2* __restrict__ ipfx, const double2* __restrict__ tpfx,
               const QueryDesc* __restrict__ desc, const int* __restrict__ item_query, int64_t item_first,
               FusedTables tab, unsigned long long* __restrict__ keys, float* __restrict__ curve_out) {
-    typedef Cfg<LOGN> C;
     constexpr int N = C::N, T = C::T, B = C::N;
     constexpr int NB = B + 1;                       // bins per spectrum row
-    // geometry: real FFT of 2B points; hop = partition length H = B/HD; an item yields the
-    // LB = 2B - H lags that the circular correlation gets right (B for HD = 1, 3B/2 for HD = 2)
-    constexpr int H = B / HD, LB = 2 * B - H, RATIO = LB / H;
+    // geometry: real FFT of 2B points; hop = partition length = B; an item yields the LB = B lags
+    // that the circular correlation gets right
+    constexpr int LB = B;
     constexpr int LAGS_PER_ROUND = T * 8;           // 8 consecutive lags per thread per round
-    constexpr int ROUNDS = LB / LAGS_PER_ROUND;     // 4 or 6
+    constexpr int ROUNDS = LB / LAGS_PER_ROUND;     // 4
     constexpr int KEEP3 = C::R3 * LB / (2 * B);     // outputs of a last-pass butterfly that carry valid lags
     static_assert(LB % LAGS_PER_ROUND == 0 && ROUNDS * 8 <= 64, "epilogue tiling");
     constexpr int NW = T / 32;
@@ -93,7 +94,7 @@ k_match_fused(const float2* __restrict__ That, int64_t part_first, const float2*
     // ---------------- 1+2. spectral multiply-accumulate and Hermitian packing ---------------
     {
         int P = d.P;
-        const int64_t row0 = k * RATIO;             // block-spectrum row of partition 0 (rows are H apart)
+        const int64_t row0 = k;                     // block-spectrum row of partition 0
         if (row0 + P > nblk) P = (int)(nblk - row0);    // rows past the end of the stream are zero
         const float2* tp = That + (d.partBase - part_first) * (int64_t)NB;
         const float2* xp = Xhat + row0 * (int64_t)NB;
@@ -153,7 +154,7 @@ k_match_fused(const float2* __restrict__ That, int64_t part_first, const float2*
     __syncthreads();
 
     // ---------------- 3. inverse FFT of N complex points in shared memory -------------------
-    ifft_smem<LOGN, KEEP3, true>(buf, s_t2, s_a3, s_b3);
+    ifft_smem<KEEP3, true>(buf, s_t2, s_a3, s_b3);
     // now buf[pad(i)] = (x[2i], x[2i+1]) for i < N/2: correlation at lags 2i, 2i+1 (times 2B)
 
     // ---------------- 4. window sums, fp32 screening, fp64 exact evaluation -----------------
@@ -316,13 +317,12 @@ k_match_fused(const float2* __restrict__ That, int64_t part_first, const float2*
 // Rows are either the lag blocks of a stream (MODE 0: samples [kB, kB+2B), centred on the stream
 // mean) or the partitions of the batch's templates (MODE 1: B samples + B zeros, centred on the
 // template's own mean) -- the gather, the centring and the FFT are one pass over the data.
-template <int LOGN, typename S, int MODE, int HD>
-__global__ void __launch_bounds__(Cfg<LOGN>::T, Cfg<LOGN>::MINB)
+template <typename S, int MODE>
+__global__ void __launch_bounds__(C::T, C::MINB)
 k_forward_rows(const S* __restrict__ src, int64_t src_n, const double2* __restrict__ pfx,
                const QueryDesc* __restrict__ desc, int q_begin, int q_end, int64_t row_first,
                FusedTables tab, float2* __restrict__ out) {
-    typedef Cfg<LOGN> C;
-    constexpr int N = C::N, T = C::T, B = C::N, NB = B + 1, H = B / HD;   // rows are H samples apart
+    constexpr int N = C::N, T = C::T, B = C::N, NB = B + 1;   // rows are B samples apart
     constexpr int NT2 = C::R2 * 32, NT3 = C::R3 * 32;
     extern __shared__ __align__(16) unsigned char smem_raw[];
     float2* buf = reinterpret_cast<float2*>(smem_raw);
@@ -338,7 +338,7 @@ k_forward_rows(const S* __restrict__ src, int64_t src_n, const double2* __restri
     float centre;
     const int64_t row = row_first + blockIdx.x;
     if (MODE == 0) {
-        off = row * H;
+        off = row * B;
         len = src_n - off; if (len > 2 * B) len = 2 * B; if (len < 0) len = 0;
         centre = Acc<S>::centre(pfx[src_n].x, (double)src_n);
     } else {
@@ -349,9 +349,9 @@ k_forward_rows(const S* __restrict__ src, int64_t src_n, const double2* __restri
         }
         __syncthreads();
         const QueryDesc d = desc[s_q];
-        const int64_t seg0 = (row - d.partBase) * H;
+        const int64_t seg0 = (row - d.partBase) * B;
         off = d.toff + seg0;
-        len = d.tlen - seg0; if (len > H) len = H;
+        len = d.tlen - seg0; if (len > B) len = B;
         centre = Acc<S>::centre(pfx[d.toff + d.tlen].x - pfx[d.toff].x, (double)d.tlen);
     }
     const S* x = src + off;
@@ -363,7 +363,7 @@ k_forward_rows(const S* __restrict__ src, int64_t src_n, const double2* __restri
         buf[pad(n)] = make_float2(a, -b);            // conj(z[n])
     }
     __syncthreads();
-    ifft_smem<LOGN, C::R3, false>(buf, s_t2, s_a3, s_b3);   // buf = conj(Z)
+    ifft_smem<C::R3, false>(buf, s_t2, s_a3, s_b3);   // buf = conj(Z)
     float2* o = out + (int64_t)blockIdx.x * NB;
     for (int k = tid; k <= B / 2; k += T) {
         const float2 zk = buf[pad(k)];
@@ -379,28 +379,25 @@ k_forward_rows(const S* __restrict__ src, int64_t src_n, const double2* __restri
     }
 }
 
-template <int LOGN> size_t forward_smem_bytes() {
-    typedef Cfg<LOGN> C;
+size_t forward_smem_bytes() {
     return ((size_t)(C::N + (C::N >> 5) + 1) + C::R2 * 32 + 2 * C::R3 * 32) * sizeof(float2) + 64;
 }
 
 // ---------------------------------------------------------------- host side
-template <int LOGN, int HD> size_t fused_smem_bytes() {
-    typedef Cfg<LOGN> C;
+size_t fused_smem_bytes() {
     const size_t padded = (size_t)(C::N + (C::N >> 5) + 1);
     const size_t nw = C::T / 32;
-    const size_t LB = 2 * C::N - C::N / HD;
+    const size_t LB = C::N;
     const size_t rounds = LB / (C::T * 8);
     return (padded + C::R2 * 32 + 2 * C::R3 * 32) * sizeof(float2) + nw * sizeof(unsigned long long)
          + 16 + rounds * nw * 2 * sizeof(double2) + (LB + 16) + (LB + 48) + 8 + nw * sizeof(float) + 64;
 }
 
 struct TableSet { float2* dev = nullptr; FusedTables tab; };
-TableSet g_tables[2];     // [0]: LOGN 13, [1]: LOGN 14
+TableSet g_tables;
 
-template <int LOGN> int ensure_tables(FusedTables* out) {
-    typedef Cfg<LOGN> C;
-    TableSet& ts = g_tables[LOGN - 13];
+int ensure_tables(FusedTables* out) {
+    TableSet& ts = g_tables;
     if (!ts.dev) {
         const int N = C::N;
         const size_t nw = N / 2 + 1, n2 = (size_t)C::R2 * 32, n3 = (size_t)C::R3 * 32;
@@ -438,17 +435,17 @@ __global__ void k_fill_item_query(const QueryDesc* __restrict__ desc, int q_begi
 int* g_item_query = nullptr;
 int64_t g_item_query_cap = 0;
 
-template <int LOGN, typename S, int HD>
+template <typename S>
 int launch_typed(const sb_stream* image, const sb_stream* tmpl, const float2* d_parts, int64_t part_first, const float2* d_premac,
                  const QueryDesc* d_desc, int q_begin, int q_end, int64_t item_first, int64_t n_items,
                  unsigned long long* d_keys, float* d_curve) {
     Ctx& c = ctx();
     FusedTables tab;
-    SB_TRY(ensure_tables<LOGN>(&tab));
+    SB_TRY(ensure_tables(&tab));
     static bool attr_set = false;
-    const size_t smem = fused_smem_bytes<LOGN, HD>();
+    const size_t smem = fused_smem_bytes();
     if (!attr_set) {
-        SB_CUDA(cudaFuncSetAttribute(k_match_fused<LOGN, S, HD>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem));
+        SB_CUDA(cudaFuncSetAttribute(k_match_fused<S>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem));
         attr_set = true;
     }
     if (g_item_query_cap < n_items) {
@@ -462,8 +459,8 @@ int launch_typed(const sb_stream* image, const sb_stream* tmpl, const float2* d_
     const int64_t max_grid = 1 << 30;
     for (int64_t i0 = 0; i0 < n_items; i0 += max_grid) {
         const int64_t ni = std::min<int64_t>(max_grid, n_items - i0);
-        k_match_fused<LOGN, S, HD><<<(unsigned)ni, Cfg<LOGN>::T, smem, c.stream>>>(
-            d_parts, part_first, d_premac ? d_premac + i0 * (int64_t)(Cfg<LOGN>::N + 1) : nullptr, image->d_spec, image->nblk,
+        k_match_fused<S><<<(unsigned)ni, C::T, smem, c.stream>>>(
+            d_parts, part_first, d_premac ? d_premac + i0 * (int64_t)(C::N + 1) : nullptr, image->d_spec, image->nblk,
             static_cast<const S*>(image->d_raw), image->n,
             image->d_pfx, tmpl->d_pfx, d_desc, g_item_query + i0, item_first + i0,
             tab, d_keys, d_curve);
@@ -472,72 +469,58 @@ int launch_typed(const sb_stream* image, const sb_stream* tmpl, const float2* d_
     return SB_OK;
 }
 
-template <int LOGN, typename S, int MODE, int HD>
+template <typename S, int MODE>
 int launch_forward_typed(const sb_stream* src, const QueryDesc* d_desc, int q_begin, int q_end,
                          int64_t row_first, int64_t rows, float2* out) {
     Ctx& c = ctx();
     FusedTables tab;
-    SB_TRY(ensure_tables<LOGN>(&tab));
+    SB_TRY(ensure_tables(&tab));
     static bool attr_set = false;
-    const size_t smem = forward_smem_bytes<LOGN>();
+    const size_t smem = forward_smem_bytes();
     if (!attr_set) {
-        SB_CUDA(cudaFuncSetAttribute(k_forward_rows<LOGN, S, MODE, HD>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem));
+        SB_CUDA(cudaFuncSetAttribute(k_forward_rows<S, MODE>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem));
         attr_set = true;
     }
-    k_forward_rows<LOGN, S, MODE, HD><<<(unsigned)rows, Cfg<LOGN>::T, smem, c.stream>>>(
+    k_forward_rows<S, MODE><<<(unsigned)rows, C::T, smem, c.stream>>>(
         static_cast<const S*>(src->d_raw), src->n, src->d_pfx, d_desc, q_begin, q_end, row_first, tab, out);
     SB_CUDA(cudaGetLastError());
     return SB_OK;
 }
 
 template <int MODE>
-int launch_forward(const sb_stream* src, int hd, const QueryDesc* d_desc, int q_begin, int q_end,
+int launch_forward(const sb_stream* src, const QueryDesc* d_desc, int q_begin, int q_end,
                    int64_t row_first, int64_t rows, float2* out) {
-    const int B = ctx().B;
-    const bool u8 = src->dtype == SB_U8;
-#define SB_FWD(LOGN, S, HD) launch_forward_typed<LOGN, S, MODE, HD>(src, d_desc, q_begin, q_end, row_first, rows, out)
-    if (B == 16384) return hd == 2 ? (u8 ? SB_FWD(14, uint8_t, 2) : SB_FWD(14, float, 2)) : (u8 ? SB_FWD(14, uint8_t, 1) : SB_FWD(14, float, 1));
-    if (B == 8192)  return hd == 2 ? (u8 ? SB_FWD(13, uint8_t, 2) : SB_FWD(13, float, 2)) : (u8 ? SB_FWD(13, uint8_t, 1) : SB_FWD(13, float, 1));
-#undef SB_FWD
-    SB_FAIL(SB_EINVAL, "fused engine supports FFT half-sizes of 8192 or 16384 samples, not %d", B);
+    if (src->dtype == SB_U8) return launch_forward_typed<uint8_t, MODE>(src, d_desc, q_begin, q_end, row_first, rows, out);
+    return launch_forward_typed<float, MODE>(src, d_desc, q_begin, q_end, row_first, rows, out);
 }
 
 }  // namespace
 
 namespace sb {
 
-bool fused_supports(int B) { return B == 16384 || B == 8192; }
-
-int launch_match_fused(const sb_stream* image, const sb_stream* tmpl, int hd, const float2* d_parts, int64_t part_first, const float2* d_premac,
+int launch_match_fused(const sb_stream* image, const sb_stream* tmpl, const float2* d_parts, int64_t part_first, const float2* d_premac,
                        const QueryDesc* d_desc, int q_begin, int q_end, int64_t item_first, int64_t n_items,
                        unsigned long long* d_keys, float* d_curve) {
-    const int B = ctx().B;
-    const bool u8 = image->dtype == SB_U8;
-#define SB_FUSED(LOGN, S, HD) launch_typed<LOGN, S, HD>(image, tmpl, d_parts, part_first, d_premac, d_desc, q_begin, q_end, item_first, n_items, d_keys, d_curve)
-    if (B == 16384) return hd == 2 ? (u8 ? SB_FUSED(14, uint8_t, 2) : SB_FUSED(14, float, 2)) : (u8 ? SB_FUSED(14, uint8_t, 1) : SB_FUSED(14, float, 1));
-    if (B == 8192)  return hd == 2 ? (u8 ? SB_FUSED(13, uint8_t, 2) : SB_FUSED(13, float, 2)) : (u8 ? SB_FUSED(13, uint8_t, 1) : SB_FUSED(13, float, 1));
-#undef SB_FUSED
-    SB_FAIL(SB_EINVAL, "fused engine supports FFT half-sizes of 8192 or 16384 samples, not %d", B);
+    if (image->dtype == SB_U8)
+        return launch_typed<uint8_t>(image, tmpl, d_parts, part_first, d_premac, d_desc, q_begin, q_end, item_first, n_items, d_keys, d_curve);
+    return launch_typed<float>(image, tmpl, d_parts, part_first, d_premac, d_desc, q_begin, q_end, item_first, n_items, d_keys, d_curve);
 }
 
 // Block spectra of a stream: rows [k_first, k_first + rows) into out (row stride B+1)
-int launch_block_spectra(const sb_stream* s, int hd, int64_t k_first, int64_t rows, float2* out) {
-    return launch_forward<0>(s, hd, nullptr, 0, 0, k_first, rows, out);
+int launch_block_spectra(const sb_stream* s, int64_t k_first, int64_t rows, float2* out) {
+    return launch_forward<0>(s, nullptr, 0, 0, k_first, rows, out);
 }
 // Partition spectra of the templates of queries [q_begin, q_end): global part rows [part_first, +rows)
-int launch_part_spectra(const sb_stream* tmpl, int hd, const QueryDesc* d_desc, int q_begin, int q_end,
+int launch_part_spectra(const sb_stream* tmpl, const QueryDesc* d_desc, int q_begin, int q_end,
                         int64_t part_first, int64_t rows, float2* out) {
-    return launch_forward<1>(tmpl, hd, d_desc, q_begin, q_end, part_first, rows, out);
+    return launch_forward<1>(tmpl, d_desc, q_begin, q_end, part_first, rows, out);
 }
 
-int fused_tables(int logn, FusedTables* out) {
-    if (logn == 14) return ensure_tables<14>(out);
-    if (logn == 13) return ensure_tables<13>(out);
-    SB_FAIL(SB_EINVAL, "internal: no FFT tables for 2^%d", logn);
-}
+int fused_tables(FusedTables* out) { return ensure_tables(out); }
 
 void fused_release_tables() {
-    for (auto& t : g_tables) { if (t.dev) cudaFree(t.dev); t.dev = nullptr; }
+    if (g_tables.dev) cudaFree(g_tables.dev);
+    g_tables.dev = nullptr;
     cudaFree(g_item_query); g_item_query = nullptr; g_item_query_cap = 0;
 }
 

@@ -22,7 +22,7 @@
 //   k_match_pair    one CTA per pair of consecutive lag blocks of a query: both are multiplied at once (2P+1
 //                   spectrum-row reads instead of 4P), the second product spectrum waits in an L2-resident
 //                   park while the first is transformed -- the default for templates of two or more partitions.
-// Values agree with sb_fused.cu / the cuFFT engine to fp32 FFT rounding (~2e-7 of the curve); k_match_packed and
+// Values agree with sb_fused.cu to fp32 FFT rounding (~2e-7 of the curve); k_match_packed and
 // k_match_pair agree bit for bit.
 // Template parameters: S = sample type of the stream (uint8_t | float); EPI = body of the epilogue on uint8 streams
 // (sb_set_epilogue): 3 = default since round 2 -- run-level bounds pick the runs of 8 lags that can hold a lag block's
@@ -1272,7 +1272,7 @@ k_forward_quad(const S* __restrict__ src, int64_t src_n, const double2* __restri
             buf[pad(n)] = make_float2(a, -b);            // conj(z[n])
         }
         __syncthreads();
-        ifft_smem<14, C::R3, false>(buf, s_t2, s_a3, s_b3);   // buf = conj(Z)
+        ifft_smem<C::R3, false>(buf, s_t2, s_a3, s_b3);   // buf = conj(Z)
         // bins k and B-k from Z[k], Z[B-k]:  X[k] = Xe + conj(w^k)*Xo,  X[B-k] = conj(Xe - conj(w^k)*Xo)
         auto bins = [&](int k, float2& xk, float2& xbk) {
             const float2 zk = buf[pad(k)];
@@ -1375,7 +1375,7 @@ int launch_forward_quad_typed(const sb_stream* src, const QueryDesc* d_desc, int
                               const int2* row_list = nullptr) {
     Ctx& c = ctx();
     FusedTables tab;
-    SB_TRY(fused_tables(14, &tab));
+    SB_TRY(fused_tables(&tab));
     static bool attr_set = false;
     const size_t smem = forward_smem_bytes14();
     if (!attr_set) {
@@ -1522,8 +1522,6 @@ int launch_pair_typed(const sb_stream* image, const sb_stream* tmpl, const float
 }  // namespace
 
 namespace sb {
-
-bool packed_supports(int B) { return B == QB; }
 
 int launch_match_packed(const sb_stream* image, const sb_stream* tmpl, const float2* d_parts, int64_t part_first,
                         const QueryDesc* d_desc, int q_begin, int q_end, int64_t item_first, int64_t n_items,

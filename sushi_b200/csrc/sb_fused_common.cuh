@@ -78,6 +78,11 @@ __device__ __forceinline__ void dft_dif(float2 (&v)[R]) {
 __device__ __forceinline__ int pad(int i) { return i + (i >> 5); }
 
 // ---------------------------------------------------------------- exact per-lag value (fp64)
+// OpenCV's rule for TM_SQDIFF_NORMED (imgproc/templmatch.cpp, common_matchTemplate; behaviour pinned by
+// tests/golden): with corr the float32-rounded sum(I*T),
+//   num = max(wnd - 2*corr + tsum2, 0);  t = sqrt(wnd) * sqrt(tsum2)  (t = 0 if wnd is ~0)
+//   out = |num| < t ? num/t : 1           -> float32
+// One rsqrt replaces the sqrt+divide pair: t = p*rsqrt(p), num/t = num*rsqrt(p), p = wnd*tsum2.
 __device__ __forceinline__ float sqdiff_exact(double corr_centred, double wsum, double wsq,
                                               double a, double b, double tsum, double tsq, double n_ab) {
     const double sit = corr_centred + b * wsum + a * tsum - n_ab;

@@ -2,7 +2,6 @@
 // Nothing here is part of the ABI (see include/sushi_b200.h for that).
 #pragma once
 #include <cuda_runtime.h>
-#include <cufft.h>
 #include <stdint.h>
 #include <string>
 #include <vector>
@@ -19,9 +18,6 @@ void set_error(const char* fmt, ...);
 #define SB_FAIL(code, ...) do { sb::set_error(__VA_ARGS__); return (code); } while (0)
 #define SB_CUDA(expr) do { cudaError_t e__ = (expr); if (e__ != cudaSuccess) { \
     sb::set_error("%s failed: %s (%s:%d)", #expr, cudaGetErrorString(e__), __FILE__, __LINE__); \
-    return SB_ECUDA; } } while (0)
-#define SB_CUFFT(expr) do { cufftResult r__ = (expr); if (r__ != CUFFT_SUCCESS) { \
-    sb::set_error("%s failed: cufft error %d (%s:%d)", #expr, (int)r__, __FILE__, __LINE__); \
     return SB_ECUDA; } } while (0)
 #define SB_TRY(expr) do { int rc__ = (expr); if (rc__ != SB_OK) return rc__; } while (0)
 
@@ -42,12 +38,13 @@ struct QueryDesc {
     int64_t partBase;  // first partition spectrum of this query
     int64_t curveOff;  // where this query's curve starts in the curve buffer (curve mode only)
     int64_t groupBase; // first multiply group of this query in the batch: MAC_GROUP consecutive lag blocks (blocked class), pairs of lag blocks (direct class)
-    int32_t P;         // ceil(n / H), H = hop = partition length
-    int32_t k0;        // lag0 / LB, LB = lags per item
+    int32_t P;         // ceil(n / B): template partitions of B samples
+    int32_t k0;        // lag0 / B: first lag block (B lags per item)
     int32_t nk;        // number of lag blocks touched
     int32_t orig;      // index of this query in the caller's arrays (descriptors are in processing order)
 };
 
+constexpr int kLagBlock = 16384;  // B: lags per lag block and samples per template partition (hop B); the FFT size is 2B
 constexpr int MAC_GROUP = 8;      // lag blocks per register-blocked multiply group (sb_matcher.cu: k_mac_blocked)
 
 struct Ctx {
@@ -55,17 +52,14 @@ struct Ctx {
     int device = -1;
     int sm_count = 132;
     cudaStream_t stream = nullptr;
-    int B = 16384;                 // lag-block size (samples); FFT size is 2B
-    int chunk_items = 1024;        // items per MAC/C2R/normalise chunk (cuFFT engine)
-    int engine = 2;                // 2: packed fused kernels (sb_fused2.cu, B = 16384; default), 4 / 5: always / never pairs of lag blocks, 1: fused lag-block kernel (sb_fused.cu), 0: cuFFT pipeline
+    int engine = 2;                // 2: packed fused kernels (sb_fused2.cu; default), 4 / 5: always / never pairs of lag blocks, 1: fused lag-block kernel (sb_fused.cu)
     int premac_mode = 0;           // 0: register-blocked multiply kernel for queries whose template spans >= 12 partitions, 1: never, 2: always
     int epilogue = 3;              // body of the packed kernels on uint8 streams: 3 = run-level bounds + k_finish_runs (default), 1 = first version (sb_set_epilogue)
-    int hop_mode = 1;              // fused engine geometry: 1 = hop B (50 % of each FFT valid, default), 2 = hop B/2 (75 %), 0 = pick per batch
     int64_t max_parts = 16384;     // template partition spectra kept per super-chunk
 
     // scratch (grown on demand)
     float2* d_parts = nullptr;  int64_t parts_cap = 0;     // [parts][B+1] complex (in-place R2C)
-    float2* d_items = nullptr;  int64_t items_cap = 0;     // [items][B+1] complex (in-place C2R)
+    float2* d_items = nullptr;  int64_t items_cap = 0;     // [items][B+1] complex products of the blocked multiply (k_mac_blocked)
     QueryDesc* d_desc = nullptr; int64_t desc_cap = 0;
     int2* d_groups = nullptr; int64_t groups_cap = 0;      // (query, first local lag block) per multiply group
     unsigned long long* d_keys = nullptr; int64_t keys_cap = 0;
@@ -74,8 +68,6 @@ struct Ctx {
     // pinned staging
     QueryDesc* h_desc = nullptr; int64_t h_desc_cap = 0;
     float* h_diff = nullptr; int64_t* h_idx = nullptr; int64_t h_res_cap = 0;
-
-    std::map<std::pair<int, int64_t>, cufftHandle> plans;   // (type, batch) -> plan for size 2B
 
     // timers / profile
     cudaEvent_t t0 = nullptr, t1 = nullptr;
@@ -119,7 +111,6 @@ struct StreamEntry {
 };
 struct MultiArgs { const StreamEntry* d_streams; const int2* d_slots; int dtype; };
 
-bool packed_supports(int B);
 // multi == nullptr: one image and one template stream (the kernels compiled as before); otherwise image / tmpl are
 // ignored and every query reads its streams from the table
 int launch_match_packed(const sb_stream* image, const sb_stream* tmpl, const float2* d_parts, int64_t part_first,
@@ -135,21 +126,17 @@ int launch_part_spectra_quad(const sb_stream* tmpl, const QueryDesc* d_desc, int
                              int64_t part_first, int64_t rows, float2* out, const MultiArgs* multi = nullptr);
 void packed_release_tables();
 
-bool fused_supports(int B);
-int launch_match_fused(const sb_stream* image, const sb_stream* tmpl, int hd, const float2* d_parts, int64_t part_first, const float2* d_premac,
+int launch_match_fused(const sb_stream* image, const sb_stream* tmpl, const float2* d_parts, int64_t part_first, const float2* d_premac,
                        const QueryDesc* d_desc, int q_begin, int q_end, int64_t item_first, int64_t n_items,
                        unsigned long long* d_keys, float* d_curve);
-int launch_block_spectra(const sb_stream* s, int hd, int64_t k_first, int64_t rows, float2* out);
-int launch_part_spectra(const sb_stream* tmpl, int hd, const QueryDesc* d_desc, int q_begin, int q_end,
+int launch_block_spectra(const sb_stream* s, int64_t k_first, int64_t rows, float2* out);
+int launch_part_spectra(const sb_stream* tmpl, const QueryDesc* d_desc, int q_begin, int q_end,
                         int64_t part_first, int64_t rows, float2* out);
 void fused_release_tables();
 
 // sb_loader.cu: sb_load_pcm after its host-to-device copy (the FLAC decoder feeds it decoded int16 PCM on the device)
 int load_pcm_device(const unsigned char* d_pcm, int64_t frames, int channels, int sample_width, int framerate,
                     int sample_rate, int64_t padding, int64_t total_len, sb_stream** out_f32, const char* who);
-
-int get_plan(int type, int64_t batch, cufftHandle* out);
-void drop_plans();
 
 }  // namespace sb
 
@@ -163,13 +150,10 @@ struct sb_stream {
     unsigned long long* d_loadhist = nullptr;
     void* d_raw = nullptr;        // n samples (u8 or f32)
     double2* d_pfx = nullptr;     // [n+1] running sums: .x = sum of samples, .y = sum of squares (exact for u8)
-    // block spectra for lag-block size specB: [nblk][specB+1] complex64
+    // block spectra in the classic layout of engine 1's kernels: [nblk][B+1] complex64, row k = FFT_2B of samples [kB, kB+2B)
     float2* d_spec = nullptr;
-    int specB = 0;
-    int specHD = 1;               // hop divisor the rows were built with (row k starts at k * specB / specHD)
-    int specEngine = -1;          // engine that built d_spec (rebuilt when the engine changes)
     int64_t nblk = 0;
-    // the same rows in the quad layout of the packed kernels (B = 16384, hop B): [nblkq][kQuadRowF2] float2
+    // the same rows in the quad layout of the packed kernels: [nblkq][kQuadRowF2] float2
     float2* d_specq = nullptr;
     int64_t nblkq = 0;
     int64_t specq_lo = 0, specq_hi = 0;   // rows [specq_lo, specq_hi) of d_specq are built (on demand, per batch)

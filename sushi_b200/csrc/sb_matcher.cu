@@ -10,7 +10,13 @@
 // is the centred cross-correlation at positions kB .. kB+B-1; the un-centred
 // sum(I*T), the window energy sum(I^2) and sum(T^2) come from exact running sums,
 // and OpenCV's normalisation rule + float32 rounding + first-index argmin are
-// applied in the same kernel that reads the correlation back.
+// applied in the same kernel that runs the inverse FFT (sb_fused.cu, sb_fused2.cu).
+// Both operands are centred before the fp32 FFTs, which keeps the transform error
+// relative to the signal's variation instead of its offset: the image stream on
+// a = mean of the whole stream, every template on b = its own mean (rounded to
+// integers for uint8 data, so the centred samples stay exact).  The kernels undo
+// the centring exactly from the running sums:
+//     sum(I*T) = sum(I'T') + b*sum(I_w) + a*sum(T) - n*a*b
 #include "sb_internal.h"
 #include <algorithm>
 #include <cmath>
@@ -19,115 +25,16 @@
 #include <map>
 #include <vector>
 
-namespace sb { int ensure_spectra(sb_stream* s, int hd); int ensure_spectra_quad(sb_stream* s, int64_t k_lo, int64_t k_hi); }
+namespace sb { int ensure_spectra(sb_stream* s); int ensure_spectra_quad(sb_stream* s, int64_t k_lo, int64_t k_hi); }
 using namespace sb;
 
 namespace {
-
-// ---- centring constants ---------------------------------------------------------
-// Both operands are centred before the fp32 FFTs (it keeps the transform error relative to
-// the signal's variation instead of its offset): the image stream on a = mean of the whole
-// stream, every template on b = its own mean.  For uint8 data a and b are rounded to
-// integers so the centred samples stay exactly representable; the centring is undone
-// exactly in the normalise kernel from the running sums:
-//     sum(I*T) = sum(I'T') + b*sum(I_w) + a*sum(T) - n*a*b
-template <typename T> __device__ __forceinline__ float centre_of(double sum, double count);
-template <> __device__ __forceinline__ float centre_of<uint8_t>(double sum, double count) { return (float)rint(sum / count); }
-template <> __device__ __forceinline__ float centre_of<float>(double sum, double count) { return (float)(sum / count); }
-
-// ---- template partitions -------------------------------------------------------
-// One CTA chunk writes 2048 floats of one partition row (row stride 2B+2 floats).
-template <typename T>
-__global__ void __launch_bounds__(256)
-k_gather_parts(const T* __restrict__ tmpl, const double2* __restrict__ tpfx,
-               const QueryDesc* __restrict__ desc, int q_begin, int q_end,
-               int64_t part_first, int B, float* __restrict__ rows, int chunks_per_row) {
-    __shared__ int s_q;
-    const int64_t row = blockIdx.x / chunks_per_row;
-    const int chunk = blockIdx.x % chunks_per_row;
-    const int64_t part = part_first + row;
-    if (threadIdx.x == 0) {                         // largest q with partBase <= part
-        int lo = q_begin, hi = q_end - 1;
-        while (lo < hi) { int mid = (lo + hi + 1) >> 1; if (desc[mid].partBase <= part) lo = mid; else hi = mid - 1; }
-        s_q = lo;
-    }
-    __syncthreads();
-    const QueryDesc d = desc[s_q];
-    const float b = centre_of<T>(tpfx[d.toff + d.tlen].x - tpfx[d.toff].x, (double)d.tlen);
-    const int64_t p = part - d.partBase;
-    const int64_t seg0 = p * B;                     // offset of this partition inside the template
-    float* out = rows + row * (int64_t)(2 * B + 2);
-    const int i0 = chunk * 2048 + threadIdx.x * 2;
-#pragma unroll
-    for (int r = 0; r < 4; ++r) {
-        int i = i0 + r * 512;
-        if (i < 2 * B) {
-            float2 v;
-            v.x = (i < B && seg0 + i < d.tlen) ? (float)tmpl[d.toff + seg0 + i] - b : 0.f;
-            v.y = (i + 1 < B && seg0 + i + 1 < d.tlen) ? (float)tmpl[d.toff + seg0 + i + 1] - b : 0.f;
-            *reinterpret_cast<float2*>(out + i) = v;
-        }
-    }
-}
-
-// ---- item lookup ---------------------------------------------------------------
-__device__ __forceinline__ int find_query(const QueryDesc* __restrict__ desc, int q_begin, int q_end, int64_t item) {
-    int lo = q_begin, hi = q_end - 1;
-    while (lo < hi) { int mid = (lo + hi + 1) >> 1; if (desc[mid].itemBase <= item) lo = mid; else hi = mid - 1; }
-    return lo;
-}
-
-// ---- spectral multiply-accumulate ------------------------------------------------
-// Y[item][bin] = sum_p conj(T^[part(q,p)][bin]) * X^[k+p][bin]
-constexpr int MAC_THREADS = 256;
-constexpr int MAC_BINS = 1024;          // bins per CTA
-__global__ void __launch_bounds__(MAC_THREADS)
-k_spectral_mac(const float2* __restrict__ That, int64_t part_first, const float2* __restrict__ Xhat, int64_t nblk,
-               const QueryDesc* __restrict__ desc, int q_begin, int q_end, int64_t item_first,
-               int B, float2* __restrict__ Y, int chunks_per_item) {
-    __shared__ int s_q;
-    const int64_t it = blockIdx.x / chunks_per_item;
-    const int chunk = blockIdx.x % chunks_per_item;
-    const int64_t item = item_first + it;
-    if (threadIdx.x == 0) s_q = find_query(desc, q_begin, q_end, item);
-    __syncthreads();
-    const QueryDesc d = desc[s_q];
-    const int64_t k = d.k0 + (item - d.itemBase);
-    const int nb = B + 1;
-    int P = d.P;
-    if (k + P > nblk) P = (int)(nblk - k);          // blocks past the stream end are all zero
-    const float2* tp = That + (d.partBase - part_first) * (int64_t)nb;
-    const float2* xp = Xhat + k * (int64_t)nb;
-    float2* y = Y + it * (int64_t)nb;
-    const int b0 = chunk * MAC_BINS + threadIdx.x;
-    float2 acc[4];
-#pragma unroll
-    for (int r = 0; r < 4; ++r) acc[r] = make_float2(0.f, 0.f);
-    for (int p = 0; p < P; ++p) {
-        const float2* t = tp + (int64_t)p * nb;
-        const float2* x = xp + (int64_t)p * nb;
-#pragma unroll
-        for (int r = 0; r < 4; ++r) {
-            int b = b0 + r * MAC_THREADS;
-            if (b < nb) {
-                float2 tv = __ldg(t + b), xv = __ldg(x + b);
-                acc[r].x += tv.x * xv.x + tv.y * xv.y;
-                acc[r].y += tv.x * xv.y - tv.y * xv.x;
-            }
-        }
-    }
-#pragma unroll
-    for (int r = 0; r < 4; ++r) {
-        int b = b0 + r * MAC_THREADS;
-        if (b < nb) y[b] = acc[r];
-    }
-}
 
 // ---- register-blocked spectral multiply for long templates ------------------------------------
 // G = MAC_GROUP consecutive lag blocks of one query share every template row: block g at partition
 // step p needs spectrum row k0+g+p, so a ring of G row values slides by one row per step and each
 // step costs one template load and ONE new spectrum load per bin for G multiply-accumulates (the
-// per-item kernel loads 2 per multiply-accumulate).  Y[item][bin] goes to a buffer the fused kernel
+// fused kernel's own multiply loads 2 per multiply-accumulate).  Y[item][bin] goes to a buffer the fused kernel
 // then reads instead of multiplying itself.  Rows are requested MACB_AHEAD steps early.
 __global__ void k_fill_groups(const QueryDesc* __restrict__ desc, int q_begin, int64_t group_first, int2* __restrict__ groups) {
     const int q = q_begin + blockIdx.x;
@@ -191,153 +98,6 @@ k_mac_blocked(const float2* __restrict__ That, int64_t part_first, const float2*
         if (g < ng) y[(int64_t)g * nb] = acc[g];
 }
 
-// ---- normalise + argmin ----------------------------------------------------------
-// OpenCV's rule for TM_SQDIFF_NORMED (imgproc/templmatch.cpp, common_matchTemplate;
-// behaviour pinned by tests/golden): with corr the float32-rounded sum(I*T),
-//   num = max(wnd - 2*corr + tsum2, 0);  t = sqrt(wnd) * sqrt(tsum2)  (t = 0 if wnd is ~0)
-//   out = |num| < t ? num/t : 1           -> float32
-// One rsqrt replaces the sqrt+divide pair: t = p*rsqrt(p), num/t = num*rsqrt(p), p = wnd*tsum2.
-__device__ __forceinline__ float sqdiff_normed(double corr_centred, double wsum, double wsq,
-                                               double a, double b, double tsum, double tsq, double n_ab) {
-    // undo the centring: sum(I*T) = sum(I'T') + b*sum(I_w) + a*sum(T) - n*a*b
-    const double sit = corr_centred + b * wsum + a * tsum - n_ab;
-    const double corr = (double)(float)sit;
-    double num = wsq - 2.0 * corr + tsq;
-    num = fmax(num, 0.0);
-    const double p = wsq * tsq;
-    if (!(wsq > 0.0) || wsq <= fmin(0.5, 10.0 * 1.1920928955078125e-07 * wsq) || !(p > 0.0)) return 1.0f;   // t == 0
-    const double r = rsqrt(p);
-    const double t = p * r;
-    return (num < t) ? (float)(num * r) : 1.0f;
-}
-
-__device__ __forceinline__ unsigned long long pack_key(float v, unsigned int rel) {
-    return ((unsigned long long)__float_as_uint(v) << 32) | rel;     // v >= 0: bit pattern is monotone
-}
-
-// The per-lag window sums sum(I) and sum(I^2) over [j, j+n) are NOT read from the fp64
-// running-sum arrays (32 B per lag of HBM traffic); each CTA takes one exact base value
-// from them and then slides the window through its lags with a block-wide scan of
-//   delta_j = I[j+n]^k - I[j]^k,  k = 1, 2
-// computed from the raw samples (2 B per lag for uint8).  For uint8 the deltas and their
-// 2048-lag partial sums are exact in int32; for float32 streams the scan runs in fp64.
-constexpr int NORM_THREADS = 256;
-constexpr int NORM_PER = 8;                          // consecutive lags per thread
-constexpr int NORM_LAGS = NORM_THREADS * NORM_PER;   // 2048 lags per CTA
-
-template <typename T> struct Slide;
-template <> struct Slide<uint8_t> {
-    typedef int acc_t;                                // exact: |delta| <= 65025, 2048 of them < 2^31
-    static __device__ __forceinline__ int sq(uint8_t hi, uint8_t lo) { return (int)hi * hi - (int)lo * lo; }
-    static __device__ __forceinline__ int ln(uint8_t hi, uint8_t lo) { return (int)hi - (int)lo; }
-};
-template <> struct Slide<float> {
-    typedef double acc_t;
-    static __device__ __forceinline__ double sq(float hi, float lo) { return (double)hi * hi - (double)lo * lo; }
-    static __device__ __forceinline__ double ln(float hi, float lo) { return (double)hi - (double)lo; }
-};
-
-template <typename T>
-__global__ void __launch_bounds__(NORM_THREADS)
-k_normalise_argmin(const float* __restrict__ corr_rows, const T* __restrict__ img, int64_t img_n,
-                   const double2* __restrict__ ipfx, const double2* __restrict__ tpfx,
-                   const QueryDesc* __restrict__ desc, int q_begin, int q_end, int64_t item_first,
-                   int B, unsigned long long* __restrict__ keys, float* __restrict__ curve_out,
-                   int chunks_per_item) {
-    typedef typename Slide<T>::acc_t acc_t;
-    __shared__ int s_q;
-    __shared__ acc_t s_wq[NORM_THREADS / 32], s_ws[NORM_THREADS / 32];
-    __shared__ unsigned long long s_best[NORM_THREADS / 32];
-    const int64_t it = blockIdx.x / chunks_per_item;
-    const int chunk = blockIdx.x % chunks_per_item;
-    const int64_t item = item_first + it;
-    if (threadIdx.x == 0) s_q = find_query(desc, q_begin, q_end, item);
-    __syncthreads();
-    const int q = s_q;
-    const QueryDesc d = desc[q];
-    const int64_t k = d.k0 + (item - d.itemBase);
-    const int64_t n = d.tlen;
-    const int64_t jlo = d.lag0, jhi = d.lag0 + d.nlags;   // valid positions [jlo, jhi)
-    const int m_blk = chunk * NORM_LAGS;                  // first lag of this CTA inside the block row
-    const int64_t j_blk = k * B + m_blk;
-    if (m_blk >= B || j_blk >= jhi || j_blk + NORM_LAGS <= jlo) return;   // nothing valid here (uniform)
-
-    const double2 t_hi = tpfx[d.toff + n], t_lo = tpfx[d.toff];
-    const double tsum = t_hi.x - t_lo.x;
-    const double tsq = t_hi.y - t_lo.y;
-    const double a = (double)centre_of<T>(ipfx[img_n].x, (double)img_n);
-    const double b = (double)centre_of<T>(tsum, (double)n);
-    const double n_ab = (double)n * a * b;
-    const double scale = 1.0 / (double)(2 * B);      // cuFFT transforms are unnormalised
-    // the scan starts at the first lag of this CTA that can be valid, so that its base window
-    // [jb, jb+n) lies inside the stream
-    const int64_t jb = j_blk > jlo ? j_blk : jlo;
-    const double2 b_hi = ipfx[jb + n], b_lo = ipfx[jb];
-    const double base_ws = b_hi.x - b_lo.x;
-    const double base_wq = b_hi.y - b_lo.y;
-
-    // thread t owns lags j0 .. j0+7; delta_i moves the window from j0+i to j0+i+1
-    const int m0 = m_blk + threadIdx.x * NORM_PER;
-    const int64_t j0 = k * B + m0;
-    acc_t dq[NORM_PER], ds[NORM_PER];
-    acc_t tq = 0, ts = 0;
-#pragma unroll
-    for (int i = 0; i < NORM_PER; ++i) {
-        const int64_t j = j0 + i;
-        acc_t eq = 0, es = 0;
-        if (j >= jb && j + n < img_n) {               // deltas before jb are not part of the scan
-            const T lo = img[j], hi = img[j + n];
-            eq = Slide<T>::sq(hi, lo); es = Slide<T>::ln(hi, lo);
-        }
-        dq[i] = tq; ds[i] = ts;                       // exclusive prefix inside the thread
-        tq += eq; ts += es;
-    }
-    const int lane = threadIdx.x & 31, warp = threadIdx.x >> 5;
-    acc_t iq = tq, is = ts;                           // inclusive warp scan of the thread totals
-#pragma unroll
-    for (int o = 1; o < 32; o <<= 1) {
-        acc_t uq = __shfl_up_sync(0xffffffffu, iq, o), us = __shfl_up_sync(0xffffffffu, is, o);
-        if (lane >= o) { iq += uq; is += us; }
-    }
-    if (lane == 31) { s_wq[warp] = iq; s_ws[warp] = is; }
-    __syncthreads();
-    acc_t oq = iq - tq, os = is - ts;
-    for (int w = 0; w < warp; ++w) { oq += s_wq[w]; os += s_ws[w]; }
-
-    unsigned long long best = ~0ull;
-    const float* row = corr_rows + it * (int64_t)(2 * B + 2) + m0;
-    float cc[NORM_PER];
-#pragma unroll
-    for (int i = 0; i < NORM_PER; i += 2) {
-        const float2 v = (m0 + i < B) ? *reinterpret_cast<const float2*>(row + i) : make_float2(0.f, 0.f);
-        cc[i] = v.x; cc[i + 1] = v.y;
-    }
-#pragma unroll
-    for (int i = 0; i < NORM_PER; ++i) {
-        const int64_t j = j0 + i;
-        if (m0 + i < B && j >= jlo && j < jhi) {
-            const double wsq = base_wq + (double)(oq + dq[i]);
-            const double wsum = base_ws + (double)(os + ds[i]);
-            const float v = sqdiff_normed((double)cc[i] * scale, wsum, wsq, a, b, tsum, tsq, n_ab);
-            if (curve_out) curve_out[d.curveOff + (j - jlo)] = v;
-            const unsigned long long key = pack_key(v, (unsigned int)(j - jlo));
-            best = key < best ? key : best;
-        }
-    }
-#pragma unroll
-    for (int o = 16; o > 0; o >>= 1) {
-        unsigned long long other = __shfl_xor_sync(0xffffffffu, best, o);
-        best = other < best ? other : best;
-    }
-    if (lane == 0) s_best[warp] = best;
-    __syncthreads();
-    if (threadIdx.x == 0) {
-#pragma unroll
-        for (int w = 1; w < NORM_THREADS / 32; ++w) best = s_best[w] < best ? s_best[w] : best;
-        if (best != ~0ull) atomicMin(keys + q, best);
-    }
-}
-
 // keys are in processing order; results go back in the caller's order
 __global__ void k_unpack_results(const unsigned long long* __restrict__ keys, const QueryDesc* __restrict__ desc,
                                  int64_t count, float* __restrict__ diff, int64_t* __restrict__ idx) {
@@ -390,11 +150,11 @@ int check_query(const sb_stream* image, const sb_stream* tmpl, int64_t q, int64_
     return SB_OK;
 }
 
-// Whether a template of n samples takes the register-blocked multiply route (engines 1-5 at hop H = B / hd)
-bool blocked_class(int64_t n, int64_t H) {
+// Whether a template of n samples takes the register-blocked multiply route (every engine)
+bool blocked_class(int64_t n) {
     const Ctx& c = ctx();
     if (c.premac_mode == 1) return false;
-    return c.premac_mode == 2 || (n + H - 1) / H >= kBlockedFromPartitions;
+    return c.premac_mode == 2 || (n + kLagBlock - 1) / kLagBlock >= kBlockedFromPartitions;
 }
 
 // Validate + plan a batch on the host.  Fills c.h_desc[0..count) in PROCESSING order: first the queries
@@ -404,22 +164,20 @@ bool blocked_class(int64_t n, int64_t H) {
 // path.  QueryDesc::orig maps back to the caller's order; curve offsets follow the caller's order.
 int plan_batch(const StreamSet& ss, int64_t count,
                const int64_t* toff, const int64_t* tlen, const int64_t* lag0, const int64_t* nlags,
-               int hd, bool allow_blocked, int direct_group, int64_t* n_direct_out,
+               int direct_group, int64_t* n_direct_out,
                int64_t* total_items, int64_t* total_parts, int64_t* total_groups, int64_t* max_query_parts) {
     Ctx& c = ctx();
-    const int B = c.B;
-    const int64_t H = B / hd, LB = 2 * (int64_t)B - H;     // partition length / hop, lags per item
+    const int64_t B = kLagBlock;                    // partition length = hop = lags per item
     SB_CUDA(cudaEventSynchronize(c.ev_desc));       // previous batch has finished reading h_desc
     if (c.h_desc_cap < count) {
         if (c.h_desc) { cudaStreamSynchronize(c.stream); cudaFreeHost(c.h_desc); c.h_desc = nullptr; c.h_desc_cap = 0; }
         SB_CUDA(cudaMallocHost((void**)&c.h_desc, sizeof(QueryDesc) * std::max<int64_t>(count, 64)));
         c.h_desc_cap = std::max<int64_t>(count, 64);
     }
-    auto blocked = [&](int64_t n) { return allow_blocked && blocked_class(n, H); };
     int64_t n_direct = 0;
     for (int64_t q = 0; q < count; ++q) {
         SB_TRY(check_query(ss.image(q), ss.tmpl(q), q, toff[q], tlen[q], lag0[q], nlags[q]));
-        if (!blocked(tlen[q])) ++n_direct;
+        if (!blocked_class(tlen[q])) ++n_direct;
     }
     int64_t items = 0, parts = 0, maxp = 0, groups = 0;
     int64_t pos_direct = 0, pos_blocked = n_direct;
@@ -428,12 +186,12 @@ int plan_batch(const StreamSet& ss, int64_t count,
         int64_t curve_total = 0;
         for (int64_t q = 0; q < count; ++q) {
             const int64_t n = tlen[q], L = nlags[q], s = lag0[q];
-            if ((blocked(n) ? 1 : 0) == cls) {
+            if ((blocked_class(n) ? 1 : 0) == cls) {
                 QueryDesc& d = c.h_desc[cls == 0 ? pos_direct++ : pos_blocked++];
                 d.toff = toff[q]; d.tlen = n; d.lag0 = s; d.nlags = L;
-                d.P = (int32_t)((n + H - 1) / H);
-                d.k0 = (int32_t)(s / LB);
-                d.nk = (int32_t)((s + L - 1) / LB - d.k0 + 1);
+                d.P = (int32_t)((n + B - 1) / B);
+                d.k0 = (int32_t)(s / B);
+                d.nk = (int32_t)((s + L - 1) / B - d.k0 + 1);
                 d.itemBase = items; d.partBase = parts; d.orig = (int32_t)q; d.curveOff = curve_total; d.groupBase = groups;
                 groups += cls == 0 ? (d.nk + direct_group - 1) / direct_group : (d.nk + MAC_GROUP - 1) / MAC_GROUP;
                 items += d.nk; parts += d.P;
@@ -462,7 +220,7 @@ int spectra_rows_multi(const StreamSet& ss, int64_t count, StreamEntry* table, s
     for (int64_t i = 0; i < ss.n; ++i) {
         if (lo[i] == INT64_MAX) continue;
         sb_stream* s = const_cast<sb_stream*>(ss.s[i]);
-        const int64_t nblk = (s->n + c.B - 1) / c.B;
+        const int64_t nblk = (s->n + kLagBlock - 1) / kLagBlock;
         const int64_t k_lo = std::max<int64_t>(lo[i], 0), k_hi = std::min<int64_t>(hi[i], nblk);
         if (k_lo >= k_hi) continue;
         if (!s->d_specq) {
@@ -491,31 +249,17 @@ int run_batch(const StreamSet& ss, int64_t count,
     const sb_stream* tmpl = ss.tmpl(0);
     if (!ss.multi() && image->dtype != tmpl->dtype) SB_FAIL(SB_EINVAL, "image and template streams differ in sample type");
     if (count > 0x7fffffffll) SB_FAIL(SB_EINVAL, "more than 2^31 queries in one batch");
-    const int B = c.B;
-    const bool use_fused = c.engine >= 1 && fused_supports(B);
-    // Geometry of the fused engine.  hop B (default): half of every 2B-point inverse FFT is valid lags,
-    // P = ceil(n/B) partitions per item.  hop B/2: three quarters are valid (1.5x the lags per FFT) but
-    // there are twice as many partition rows to multiply and twice as many block-spectrum rows competing
-    // for L2: it pays for short templates only, so mode 0 switches only when every template is short.
-    int hd = 1;
-    if (use_fused) {
-        if (c.hop_mode == 2) hd = 2;
-        else if (c.hop_mode == 0 && c.engine == 1) {
-            int64_t longest = 0;
-            for (int64_t q = 0; q < count; ++q) longest = std::max<int64_t>(longest, tlen[q]);
-            if (longest <= B / 2) hd = 2;
-        }
-    }
+    const int B = kLagBlock;
     // Multiply strategy per query: inside the fused kernel (2 loads per multiply-accumulate, nothing through
     // HBM), or -- for very long templates (kBlockedFromPartitions) -- the register-blocked kernel
     // k_mac_blocked over MAC_GROUP lag blocks, whose products the fused kernel then reads from a chunk buffer.
-    // Engines 2 / 3: the direct class runs the packed kernels (sb_fused2.cu) on quad-layout spectrum rows (they
-    // cover B = 16384 at hop B); the blocked class keeps engine 1's kernels and the classic row layout, so a
-    // stream may hold its block spectra in both layouts.
-    const bool use_packed = c.engine >= 2 && packed_supports(B) && hd == 1;
+    // Engine 1 runs the direct class on the fused kernel of sb_fused.cu; engines 2 / 4 / 5 run it on the packed
+    // kernels (sb_fused2.cu) over quad-layout spectrum rows.  The blocked class always keeps engine 1's kernels and
+    // the classic row layout, so a stream may hold its block spectra in both layouts.
+    const bool use_packed = c.engine >= 2;
     const int nb = B + 1;                                    // float2 per classic spectrum row
     int64_t n_direct = 0, total_items = 0, total_parts = 0, total_groups = 0, maxp = 0;
-    SB_TRY(plan_batch(ss, count, toff, tlen, lag0, nlags, hd, use_fused && hd == 1, 2, &n_direct,
+    SB_TRY(plan_batch(ss, count, toff, tlen, lag0, nlags, 2, &n_direct,
                       &total_items, &total_parts, &total_groups, &maxp));
     if (ss.multi() && (!use_packed || n_direct != count)) SB_FAIL(SB_EINVAL, "internal: a multi-stream batch must be packed direct-class only");
     // Packed kernels: one CTA per lag block, or one per pair of consecutive lag blocks of a query (shared template
@@ -565,7 +309,7 @@ int run_batch(const StreamSet& ss, int64_t count,
         }
         SB_TRY(ensure_spectra_quad(image, k_lo, k_hi));
     }
-    if (!use_packed || n_direct < count) SB_TRY(ensure_spectra(image, hd));
+    if (!use_packed || n_direct < count) SB_TRY(ensure_spectra(image));
 
     SB_TRY(grow(&c.d_desc, &c.desc_cap, count));
     SB_TRY(grow(&c.d_keys, &c.keys_cap, count));
@@ -577,14 +321,8 @@ int run_batch(const StreamSet& ss, int64_t count,
     // float2 per template partition row: quad layout or classic
     const int64_t part_row_f2 = use_packed ? kQuadRowF2 : nb;
     SB_TRY(grow(&c.d_parts, &c.parts_cap, parts_cap_want * part_row_f2));
-    const int64_t chunk = std::min<int64_t>(c.chunk_items, total_items);
-    if (!use_fused) SB_TRY(grow(&c.d_items, &c.items_cap, chunk * nb));
-    // lag blocks per product buffer (0.5 GB at B = 16384)
+    // lag blocks per product buffer (0.5 GB)
     const int64_t premac_chunk = 4096;
-
-    const int gchunks = (2 * B + 2047) / 2048;
-    const int mchunks = (nb + MAC_BINS - 1) / MAC_BINS;
-    const int nchunks = (B + NORM_LAGS - 1) / NORM_LAGS;
 
     // the two query classes, each in super-chunks of whole queries whose partition spectra fit the buffer
     for (int cls = 0; cls < 2; ++cls) {
@@ -597,32 +335,10 @@ int run_batch(const StreamSet& ss, int64_t count,
         if (qe == qb) SB_FAIL(SB_ENOMEM, "internal: partition buffer too small");
         const int64_t part_first = c.h_desc[qb].partBase;
         // 1. template partitions -> spectra
-        const int64_t sub = 4096;
-        if (use_packed && !premac) {
+        {
             ProfScope ps("part_spectra");
-            SB_TRY(launch_part_spectra_quad(tmpl, c.d_desc, (int)qb, (int)qe, part_first, np, c.d_parts, mp));
-        } else if (use_fused) {                      // hand-written gather + forward FFT, one launch
-            ProfScope ps("part_spectra");
-            SB_TRY(launch_part_spectra(tmpl, hd, c.d_desc, (int)qb, (int)qe, part_first, np, c.d_parts));
-        } else
-        for (int64_t p0 = 0; p0 < np; p0 += sub) {
-            const int64_t rows = std::min<int64_t>(sub, np - p0);
-            float* dst = reinterpret_cast<float*>(c.d_parts + p0 * nb);
-            {
-                ProfScope ps("gather_parts");
-                if (tmpl->dtype == SB_U8)
-                    k_gather_parts<uint8_t><<<(unsigned)(rows * gchunks), 256, 0, c.stream>>>(
-                        static_cast<const uint8_t*>(tmpl->d_raw), tmpl->d_pfx, c.d_desc, (int)qb, (int)qe, part_first + p0, B, dst, gchunks);
-                else
-                    k_gather_parts<float><<<(unsigned)(rows * gchunks), 256, 0, c.stream>>>(
-                        static_cast<const float*>(tmpl->d_raw), tmpl->d_pfx, c.d_desc, (int)qb, (int)qe, part_first + p0, B, dst, gchunks);
-            }
-            cufftHandle plan;
-            SB_TRY(get_plan(CUFFT_R2C, rows, &plan));
-            {
-                ProfScope ps("cufft_r2c_parts", 0);
-                SB_CUFFT(cufftExecR2C(plan, dst, reinterpret_cast<cufftComplex*>(dst)));
-            }
+            if (use_packed && !premac) SB_TRY(launch_part_spectra_quad(tmpl, c.d_desc, (int)qb, (int)qe, part_first, np, c.d_parts, mp));
+            else SB_TRY(launch_part_spectra(tmpl, c.d_desc, (int)qb, (int)qe, part_first, np, c.d_parts));
         }
         // 2. items of these queries
         const int64_t item_lo = c.h_desc[qb].itemBase;
@@ -636,11 +352,11 @@ int run_batch(const StreamSet& ss, int64_t count,
             } else
                 SB_TRY(launch_match_packed(image, tmpl, c.d_parts, part_first, c.d_desc, (int)qb, (int)qe,
                                            item_lo, item_hi - item_lo, c.d_keys, d_curve, mp));
-        } else if (use_fused && !premac) {
+        } else if (!premac) {
             ProfScope ps("match_fused");
-            SB_TRY(launch_match_fused(image, tmpl, hd, c.d_parts, part_first, nullptr, c.d_desc, (int)qb, (int)qe,
+            SB_TRY(launch_match_fused(image, tmpl, c.d_parts, part_first, nullptr, c.d_desc, (int)qb, (int)qe,
                                       item_lo, item_hi - item_lo, c.d_keys, d_curve));
-        } else if (use_fused) {
+        } else {
             int64_t qa = qb;
             while (qa < qe) {
                 int64_t qz = qa, ni = 0;
@@ -658,37 +374,10 @@ int run_batch(const StreamSet& ss, int64_t count,
                 }
                 {
                     ProfScope ps("match_fused");
-                    SB_TRY(launch_match_fused(image, tmpl, hd, c.d_parts, part_first, c.d_items, c.d_desc, (int)qa, (int)qz,
+                    SB_TRY(launch_match_fused(image, tmpl, c.d_parts, part_first, c.d_items, c.d_desc, (int)qa, (int)qz,
                                               i0, ni, c.d_keys, d_curve));
                 }
                 qa = qz;
-            }
-        } else
-        for (int64_t i0 = item_lo; i0 < item_hi; i0 += chunk) {
-            const int64_t ni = std::min<int64_t>(chunk, item_hi - i0);
-            {
-                ProfScope ps("spectral_mac");
-                k_spectral_mac<<<(unsigned)(ni * mchunks), MAC_THREADS, 0, c.stream>>>(
-                    c.d_parts, part_first, image->d_spec, image->nblk, c.d_desc, (int)qb, (int)qe, i0, B, c.d_items, mchunks);
-            }
-            cufftHandle plan;
-            SB_TRY(get_plan(CUFFT_C2R, ni, &plan));
-            {
-                ProfScope ps("cufft_c2r_items", 0);
-                SB_CUFFT(cufftExecC2R(plan, reinterpret_cast<cufftComplex*>(c.d_items), reinterpret_cast<float*>(c.d_items)));
-            }
-            {
-                ProfScope ps("normalise_argmin");
-                if (image->dtype == SB_U8)
-                    k_normalise_argmin<uint8_t><<<(unsigned)(ni * nchunks), NORM_THREADS, 0, c.stream>>>(
-                        reinterpret_cast<const float*>(c.d_items), static_cast<const uint8_t*>(image->d_raw), image->n,
-                        image->d_pfx, tmpl->d_pfx,
-                        c.d_desc, (int)qb, (int)qe, i0, B, c.d_keys, d_curve, nchunks);
-                else
-                    k_normalise_argmin<float><<<(unsigned)(ni * nchunks), NORM_THREADS, 0, c.stream>>>(
-                        reinterpret_cast<const float*>(c.d_items), static_cast<const float*>(image->d_raw), image->n,
-                        image->d_pfx, tmpl->d_pfx,
-                        c.d_desc, (int)qb, (int)qe, i0, B, c.d_keys, d_curve, nchunks);
             }
         }
         qb = qe;
@@ -748,10 +437,10 @@ int curves_to_host(const StreamSet& ss, int64_t count, const int64_t* tmpl_off, 
     return rc;
 }
 
-// Multi-stream calls.  The packed engine's direct class (engines 2, 4, 5 at B = 16384, hop B; templates below the
-// blocked threshold) goes out as ONE multi-stream batch, whatever the number of streams.  Everything else -- the
-// blocked class, engines 0 / 1, other block sizes, hop B/2 -- runs as one ordinary single-stream batch per distinct
-// (image, template) pair inside the same call: same results, more launches.  Results land in the caller's order.
+// Multi-stream calls.  The packed engine's direct class (engines 2, 4, 5; templates below the blocked threshold) goes
+// out as ONE multi-stream batch, whatever the number of streams.  Everything else -- the blocked class and engine 1 --
+// runs as one ordinary single-stream batch per distinct (image, template) pair inside the same call: same results,
+// more launches.  Results land in the caller's order.
 int run_multi(const char* who, const sb_stream* const* streams, int32_t n_streams, int64_t count,
               const int32_t* image_slot, const int32_t* tmpl_slot, const int64_t* tmpl_off, const int64_t* tmpl_len,
               const int64_t* lag0, const int64_t* nlags, float* diff_out, int64_t* idx_out, float* curves_out) {
@@ -772,8 +461,7 @@ int run_multi(const char* who, const sb_stream* const* streams, int32_t n_stream
         if (tmpl_slot[q] < 0 || tmpl_slot[q] >= n_streams) SB_FAIL(SB_EINVAL, "%s: query %lld: template slot %d outside [0, %d)", who, (long long)q, (int)tmpl_slot[q], (int)n_streams);
         SB_TRY(check_query(streams[image_slot[q]], streams[tmpl_slot[q]], q, tmpl_off[q], tmpl_len[q], lag0[q], nlags[q]));
     }
-    // run_batch's geometry for these settings: the packed kernels run at hop B unless hop B/2 is forced
-    const bool packed = c.engine >= 2 && packed_supports(c.B) && c.hop_mode != 2;
+    const bool packed = c.engine >= 2;
     std::vector<int64_t> curve_off(count + 1, 0);
     for (int64_t q = 0; q < count; ++q) curve_off[q + 1] = curve_off[q] + nlags[q];
     // one subset of the queries: descriptor arrays gathered, results scattered back to the caller's positions
@@ -806,7 +494,7 @@ int run_multi(const char* who, const sb_stream* const* streams, int32_t n_stream
     std::vector<int64_t> direct;
     std::map<std::pair<int32_t, int32_t>, std::vector<int64_t>> other;
     for (int64_t q = 0; q < count; ++q) {
-        if (packed && !blocked_class(tmpl_len[q], c.B)) direct.push_back(q);
+        if (packed && !blocked_class(tmpl_len[q])) direct.push_back(q);
         else other[{image_slot[q], tmpl_slot[q]}].push_back(q);
     }
     if (!direct.empty()) {

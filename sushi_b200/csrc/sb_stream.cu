@@ -260,31 +260,6 @@ k_tile_scan_u8(const uint8_t* __restrict__ x, int64_t n, const uint2* __restrict
     }
 }
 
-// Centred float rows for the block spectra: row k holds image[kB .. kB+2B) - c,
-// zero beyond the end of the stream; rows are (2B+2) floats apart (in-place R2C).
-template <typename T>
-__global__ void __launch_bounds__(256)
-k_gather_blocks(const T* __restrict__ x, int64_t n, const double2* __restrict__ pfx, int B, float* __restrict__ rows,
-                int64_t k_first, int chunks_per_row) {
-    const float c = sizeof(T) == 1 ? (float)rint(pfx[n].x / (double)n) : (float)(pfx[n].x / (double)n);   // = centre_of<T>
-    const int64_t row = blockIdx.x / chunks_per_row;
-    const int chunk = blockIdx.x % chunks_per_row;
-    const int64_t k = k_first + row;
-    float* out = rows + row * (int64_t)(2 * B + 2);
-    const int i0 = chunk * 2048 + threadIdx.x * 2;
-#pragma unroll
-    for (int r = 0; r < 4; ++r) {
-        int i = i0 + r * 512;
-        if (i < 2 * B) {
-            int64_t j = k * B + i;
-            float2 v;
-            v.x = j < n ? (float)x[j] - c : 0.f;
-            v.y = j + 1 < n ? (float)x[j + 1] - c : 0.f;
-            *reinterpret_cast<float2*>(out + i) = v;
-        }
-    }
-}
-
 constexpr size_t kTotSmem = 2 * sizeof(double) * (TOT_SLAB + TOT_SLAB / TOT_ITEMS);
 int ensure_tot_smem() {
     static bool attr_set = false;
@@ -385,9 +360,7 @@ int stream_finish_public(sb_stream* s) { return stream_finish(s); }
 // touches only the part of the destination stream its own events' search windows cover, so it transforms
 // that part only (the replicated stream preparation is the Amdahl term of strong scaling, SURVEY.md 8e).
 int ensure_spectra_quad(sb_stream* s, int64_t k_lo, int64_t k_hi) {
-    Ctx& c = ctx();
-    if (!packed_supports(c.B)) SB_FAIL(SB_EINVAL, "internal: quad-layout spectra need a lag block of 16384");
-    const int64_t nblk = (s->n + c.B - 1) / c.B;
+    const int64_t nblk = (s->n + kLagBlock - 1) / kLagBlock;
     if (k_lo < 0) k_lo = 0;
     if (k_hi > nblk) k_hi = nblk;
     if (k_lo >= k_hi) return SB_OK;
@@ -411,49 +384,20 @@ int ensure_spectra_quad(sb_stream* s, int64_t k_lo, int64_t k_hi) {
     return SB_OK;
 }
 
-// Build (or fetch) the block spectra of `s`: row k = FFT_2B of samples [k*H, k*H + 2B), H = B/hd.
-int ensure_spectra(sb_stream* s, int hd) {
-    Ctx& c = ctx();
-    // classic row layout ([B+1] complex per row): engine 1's kernels (also behind engines 2 / 3 for the
-    // queries routed through the blocked multiply) or the cuFFT pipeline
-    const int eng = (c.engine >= 1 && fused_supports(c.B)) ? 1 : 0;
-    if (s->d_spec && s->specB == c.B && s->specHD == hd && s->specEngine == eng) return SB_OK;
-    if (s->d_spec) { pool_free(s->d_spec); s->d_spec = nullptr; }
-    const int B = c.B, H = B / hd;
-    const int64_t nblk = (s->n + H - 1) / H;
-    SB_TRY(pool_alloc((void**)&s->d_spec, sizeof(float2) * (size_t)nblk * (B + 1)));
-    if (c.engine >= 1 && fused_supports(B)) {        // hand-written gather + forward FFT, one launch
-        {
-            ProfScope ps("block_spectra");
-            SB_TRY(launch_block_spectra(s, hd, 0, nblk, s->d_spec));
-        }
-        s->specB = B; s->specHD = hd; s->nblk = nblk; s->specEngine = 1;
-        return SB_OK;
+// Build (or fetch) the block spectra of `s` in the classic row layout of engine 1's kernels (also behind engines
+// 2 / 4 / 5 for the queries routed through the blocked multiply): row k = FFT_2B of samples [kB, kB + 2B).
+int ensure_spectra(sb_stream* s) {
+    if (s->d_spec) return SB_OK;
+    const int64_t nblk = (s->n + kLagBlock - 1) / kLagBlock;
+    float2* spec = nullptr;
+    SB_TRY(pool_alloc((void**)&spec, sizeof(float2) * (size_t)nblk * (kLagBlock + 1)));
+    int rc;
+    {
+        ProfScope ps("block_spectra");
+        rc = launch_block_spectra(s, 0, nblk, spec);
     }
-    if (hd != 1) SB_FAIL(SB_EINVAL, "internal: the cuFFT engine only builds spectra at hop B");
-    const int chunks = (2 * B + 2047) / 2048;
-    const int64_t sub = 1024;                        // rows per cuFFT call
-    for (int64_t k = 0; k < nblk; k += sub) {
-        const int64_t rows = (nblk - k) < sub ? (nblk - k) : sub;
-        float* dst = reinterpret_cast<float*>(s->d_spec + k * (B + 1));
-        {
-            ProfScope ps("gather_blocks");
-            if (s->dtype == SB_U8)
-                k_gather_blocks<uint8_t><<<(unsigned)(rows * chunks), 256, 0, c.stream>>>(
-                    static_cast<const uint8_t*>(s->d_raw), s->n, s->d_pfx, B, dst, k, chunks);
-            else
-                k_gather_blocks<float><<<(unsigned)(rows * chunks), 256, 0, c.stream>>>(
-                    static_cast<const float*>(s->d_raw), s->n, s->d_pfx, B, dst, k, chunks);
-        }
-        cufftHandle plan;
-        SB_TRY(get_plan(CUFFT_R2C, rows, &plan));
-        {
-            ProfScope ps("cufft_r2c_blocks", 0);
-            SB_CUFFT(cufftExecR2C(plan, dst, reinterpret_cast<cufftComplex*>(dst)));
-        }
-    }
-    SB_CUDA(cudaGetLastError());
-    s->specB = B; s->specHD = 1; s->nblk = nblk; s->specEngine = 0;
+    if (rc != SB_OK) { pool_free(spec); return rc; }
+    s->d_spec = spec; s->nblk = nblk;
     return SB_OK;
 }
 

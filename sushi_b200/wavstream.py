@@ -694,9 +694,8 @@ class WavStream(StreamGeometry):
         start + anchor with +-window (the fast path, sushi.py:431-432).  Precompute, in ONE launch, the
         curves of the next groups over a slightly wider span; find_substream then answers from them.
         A curve value depends only on (template, absolute position), so a cached curve answers any
-        contained range with exactly the value and first-index argmin a live call returns (the packed
-        engines at hop B, the default, compute a value the same way whatever the batch; the
-        first-generation engine with hop_mode 0 picks its geometry per batch and agrees only to ~1e-7)."""
+        contained range with exactly the value and first-index argmin a live call returns (every engine
+        computes a value the same way whatever the batch)."""
         plan = self._speculation_plan(src_stream, groups, idx, anchor, window)
         if plan is not None:
             self._fill_curve_cache(src_stream, plan, self.match_curves(src_stream, *plan))

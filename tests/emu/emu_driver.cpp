@@ -157,7 +157,7 @@ int emu_run_slots(void) { return kRunSlots; }
 int emu_run_record_bytes(void) { return (int)sizeof(RunRecord); }
 
 // Block spectra of a stream (k_forward_quad, MODE 0): rows [row_first, row_first + rows) into
-// `out` (rows * emu_quad_row_floats() floats).  The twiddle tables are the ones sb_fused.cu's ensure_tables<14>
+// `out` (rows * emu_quad_row_floats() floats).  The twiddle tables are the ones sb_fused.cu's ensure_tables
 // builds.
 int emu_forward_blocks(int is_u8, const void* src, int64_t src_n, const double* pfx, int64_t row_first, int rows, float* out) {
     typedef Cfg<14> C;

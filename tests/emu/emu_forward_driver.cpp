@@ -6,7 +6,7 @@
 #include "emu_multi_driver.cpp"
 
 namespace {
-// The twiddle tables sb_fused.cu's ensure_tables<14> builds (the same values as emu_forward_blocks)
+// The twiddle tables sb_fused.cu's ensure_tables builds (the same values as emu_forward_blocks)
 const FusedTables& walk_tables() {
     typedef Cfg<14> C;
     static std::vector<float2> h;

@@ -13,7 +13,7 @@ reproduce and the closed form does not, moves a value by at most 2^-24 * 2 sum(I
 depends on the template length: the rounding of a correlation value is proportional to the norm of the whole 2B-point
 block times the template's norm, while the value is divided by the window's and the template's energies, so it grows
 like sqrt(2B / n).  Templates of fewer than SHORT samples therefore get 1e-6 * sqrt(SHORT / n) (2.8e-6 at n = 2, where
-the cuFFT engine measured 1.4e-6 on white noise).  The worst error per setting and sample type is printed at the end
+a since retired cuFFT engine measured 1.4e-6 on white noise).  The worst error per setting and sample type is printed at the end
 of the module (run with -s to see it)."""
 import ctypes
 import collections
@@ -26,28 +26,23 @@ from tests import closed_form_cases as cf
 
 pytestmark = pytest.mark.gpu
 
-B = cf.B
 VALUE_TOL = 1e-6
 SHORT = 16
 ARGMIN_TOL = 2e-6
 
-Setting = collections.namedtuple('Setting', 'name engine hop premac epilogue block max_parts')
-DEFAULTS = Setting('default', 2, 1, 0, 3, B, 16384)
+Setting = collections.namedtuple('Setting', 'name engine premac epilogue max_parts')
+DEFAULTS = Setting('default', 2, 0, 3, 16384)
 SETTINGS = [
-    Setting('cufft', 0, 1, 0, 3, B, 16384),
-    Setting('cufft_b8192', 0, 1, 0, 3, 8192, 16384),
-    Setting('fused_hop1', 1, 1, 0, 3, B, 16384),
-    Setting('fused_hop1_b8192', 1, 1, 0, 3, 8192, 16384),
-    Setting('fused_hop2', 1, 2, 0, 3, B, 16384),
-    Setting('fused_blocked', 1, 1, 2, 3, B, 16384),
-    Setting('packed_epi3', 2, 1, 0, 3, B, 16384),
-    Setting('packed_epi1', 2, 1, 0, 1, B, 16384),
-    Setting('pairs_epi3', 4, 1, 0, 3, B, 16384),
-    Setting('pairs_epi1', 4, 1, 0, 1, B, 16384),
-    Setting('single_epi3', 5, 1, 0, 3, B, 16384),
-    Setting('single_epi1', 5, 1, 0, 1, B, 16384),
-    Setting('packed_passes', 2, 1, 0, 3, B, 1),                  # every query in a launch pass of its own
-    Setting('fused_passes_b8192', 1, 1, 0, 3, 8192, 1),
+    Setting('fused_hop1', 1, 0, 3, 16384),
+    Setting('fused_blocked', 1, 2, 3, 16384),
+    Setting('packed_epi3', 2, 0, 3, 16384),
+    Setting('packed_epi1', 2, 0, 1, 16384),
+    Setting('pairs_epi3', 4, 0, 3, 16384),
+    Setting('pairs_epi1', 4, 0, 1, 16384),
+    Setting('single_epi3', 5, 0, 3, 16384),
+    Setting('single_epi1', 5, 0, 1, 16384),
+    Setting('packed_passes', 2, 0, 3, 1),                        # every query in a launch pass of its own
+    Setting('fused_passes', 1, 0, 3, 1),
 ]
 
 CASES = cf.all_cases()
@@ -55,8 +50,8 @@ WORST = collections.defaultdict(float)          # (setting, dtype[, 'n < SHORT']
 
 
 def apply(lib, s):
-    for rc in (lib.sb_set_block_size(s.block), lib.sb_set_engine(s.engine), lib.sb_set_hop_mode(s.hop),
-               lib.sb_set_premac_mode(s.premac), lib.sb_set_epilogue(s.epilogue), lib.sb_set_max_parts(s.max_parts)):
+    for rc in (lib.sb_set_engine(s.engine), lib.sb_set_premac_mode(s.premac), lib.sb_set_epilogue(s.epilogue),
+               lib.sb_set_max_parts(s.max_parts)):
         _native.check(rc)
 
 

@@ -57,67 +57,62 @@ def test_whole_curve_matches_reference_golden(gpu_lib, golden_matcher, pair, sty
 
 
 @pytest.mark.parametrize('stype', ['uint8', 'float32'])
-@pytest.mark.parametrize('block', [1024, 4096, 8192, 16384])
-def test_live_oracle_random_queries(gpu_lib, pair, stype, block):
-    """Random (event, centre, window) queries: GPU vs the oracle's cv2 call, for several lag-block
-    sizes (every size must give the same answer: values do not depend on the blocking)."""
+@pytest.mark.parametrize('seed', [1024, 4096, 8192, 16384], ids=lambda v: 'seed%d' % v)
+def test_live_oracle_random_queries(gpu_lib, pair, stype, seed):
+    """Random (event, centre, window) queries: GPU vs the oracle's cv2 call, 12 per seed."""
     rs, rd, src, dst = pair[stype]
-    _native.check(gpu_lib.sb_set_block_size(block))
-    try:
-        rng = np.random.default_rng(block)
-        for _ in range(12):
-            a = float(rng.uniform(0.0, 20.0))
-            ln = float(rng.choice([0.05, 0.5, 1.0, 3.0, 3.9]))
-            b = min(a + ln, 24.0)
-            c = float(a + rng.uniform(-3, 3))
-            w = float(rng.choice([0.3, 1.5, 5.0, 10.0, 30.0]))
-            pat_ref = rs.get_substream(a, b)
-            d_ref, t_ref = rd.find_substream(pat_ref, c, w)
-            d, t = dst.find_substream(src.get_substream(a, b), c, w)
-            assert abs(float(d) - float(d_ref)) <= DIFF_TOL, (a, b, c, w)
-            assert abs(t - t_ref) <= SHIFT_TOL, (a, b, c, w, t, t_ref)
-    finally:
-        _native.check(gpu_lib.sb_set_block_size(16384))
+    rng = np.random.default_rng(seed)
+    for _ in range(12):
+        a = float(rng.uniform(0.0, 20.0))
+        ln = float(rng.choice([0.05, 0.5, 1.0, 3.0, 3.9]))
+        b = min(a + ln, 24.0)
+        c = float(a + rng.uniform(-3, 3))
+        w = float(rng.choice([0.3, 1.5, 5.0, 10.0, 30.0]))
+        pat_ref = rs.get_substream(a, b)
+        d_ref, t_ref = rd.find_substream(pat_ref, c, w)
+        d, t = dst.find_substream(src.get_substream(a, b), c, w)
+        assert abs(float(d) - float(d_ref)) <= DIFF_TOL, (a, b, c, w)
+        assert abs(t - t_ref) <= SHIFT_TOL, (a, b, c, w, t, t_ref)
 
 
 @pytest.mark.parametrize('stype', ['uint8', 'float32'])
-@pytest.mark.parametrize('block', [8192, 16384])
-def test_fused_engine_equals_cufft_engine(gpu_lib, pair, stype, block):
-    """The fused kernel and the cuFFT-planned pipeline are two implementations of the same
-    formulation: whole curves agree to float32 FFT noise, batch results to the tolerance."""
+@pytest.mark.parametrize('n', [11400, 40000], ids=['one_partition', 'three_partitions'])
+def test_engines_agree_with_the_closed_form_and_each_other(gpu_lib, pair, stype, n):
+    """Every engine is an implementation of the same formulation: each one's whole curve is within 1e-6 of the
+    fp64 closed form, the engines agree with each other to float32 FFT noise, and each batch result is the
+    first-index minimum of the engine's own curve -- for a template of one partition and one of three."""
+    from oracle.ref_matcher import sqdiff_normed_fp64
     rs, rd, src, dst = pair[stype]
-    _native.check(gpu_lib.sb_set_block_size(block))
     try:
-        toff, n = src._get_sample_for_time(6.1), 11400
+        toff = src._get_sample_for_time(6.1)
         lag0, nlags = 70000, 150001
+        truth = sqdiff_normed_fp64(dst.data[0, lag0:lag0 + nlags + n - 1], src.data[0, toff:toff + n])
         curves, results = [], []
-        # (engine, hop mode): the cuFFT pipeline, then the fused kernel in both overlap-save geometries
-        # + the fused kernel fed by the register-blocked multiply kernel (premac 2 = for every query)
-        # + the packed fused kernels (engine 2 picks per batch between one CTA per lag block = engine 5 and one
-        # CTA per pair of lag blocks with the second product spectrum parked in L2 = engine 4;
-        # they cover B = 16384 and fall back to engine 1 otherwise)
-        variants = [(0, 1, 1), (1, 1, 1), (1, 2, 1), (1, 1, 2), (2, 1, 1), (4, 1, 1), (5, 1, 1)]
-        for engine, hop, premac in variants:
+        # (engine, premac mode): the fused kernel, the fused kernel fed by the register-blocked multiply kernel
+        # (premac 2 = for every query), the packed fused kernels (engine 2 picks per batch between one CTA per
+        # lag block = engine 5 and one CTA per pair of lag blocks with the second product spectrum parked in
+        # L2 = engine 4)
+        variants = [(1, 1), (1, 2), (2, 1), (4, 1), (5, 1)]
+        for engine, premac in variants:
             _native.check(gpu_lib.sb_set_engine(engine))
-            _native.check(gpu_lib.sb_set_hop_mode(hop))
             _native.check(gpu_lib.sb_set_premac_mode(premac))
             curves.append(dst.match_curve(src, toff, n, lag0, nlags))
+            assert np.abs(curves[-1] - truth).max() <= 1e-6, (engine, premac)
             results.append(dst.find_planned(src, [toff, toff + 5000, 100], [n, 3000, 48000],
                                             [lag0, 1000, 0], [nlags, 300000, 200000]))
             # the batch result is the first-index minimum of the variant's own curve
             d, i = dst.find_planned(src, [toff], [n], [lag0], [nlags])
             assert i[0] == int(curves[-1].argmin()) and d[0] == curves[-1].min()
-        for e in (1, 2, 3, 4, 5, 6):
-            assert np.abs(curves[0] - curves[e]).max() <= 2e-6
-            assert np.abs(results[0][0] - results[e][0]).max() <= 2e-6
-            assert np.abs(results[0][1] - results[e][1]).max() <= 1
+        for a in range(len(variants)):
+            for b in range(a + 1, len(variants)):
+                assert np.abs(curves[a] - curves[b]).max() <= 2e-6, (variants[a], variants[b])
+                assert np.abs(results[a][0] - results[b][0]).max() <= 2e-6, (variants[a], variants[b])
+                assert np.abs(results[a][1] - results[b][1]).max() <= 1, (variants[a], variants[b])
         # pairs or single lag blocks (engines 4 / 5): the same arithmetic in the same order
-        assert np.array_equal(curves[5], curves[6]) and np.array_equal(results[5][0], results[6][0])
+        assert np.array_equal(curves[3], curves[4]) and np.array_equal(results[3][0], results[4][0])
     finally:
         _native.check(gpu_lib.sb_set_engine(2))
-        _native.check(gpu_lib.sb_set_hop_mode(1))
         _native.check(gpu_lib.sb_set_premac_mode(0))
-        _native.check(gpu_lib.sb_set_block_size(16384))
 
 
 def test_raw_ndarray_pattern_and_halves(gpu_lib, pair):
@@ -336,14 +331,13 @@ def test_empty_batch_is_a_no_op(gpu_lib, pair):
     assert len(d) == 0 and len(i) == 0
 
 
-@pytest.mark.parametrize('engine', [0, 1, 2, 3, 4, 6, 7])
+@pytest.mark.parametrize('engine', [1, 3, 4, 6, 7])
 def test_minimum_sizes_and_ragged_edges(gpu_lib, engine):
     """n = 1 templates, single-lag searches, streams shorter than one lag block, searches that end on
     the last sample, spans that straddle exactly one block boundary."""
     rng = np.random.default_rng(engine)
-    # 2 = fused kernel at hop B/2, 3 = blocked multiply, 4 / 6 / 7 = packed fused kernels (library engines 2 / 4 / 5)
-    _native.check(gpu_lib.sb_set_engine(engine - 2 if engine >= 4 else min(engine, 1)))
-    _native.check(gpu_lib.sb_set_hop_mode(2 if engine == 2 else 1))
+    # 1 = fused kernel, 3 = blocked multiply, 4 / 6 / 7 = packed fused kernels (library engines 2 / 4 / 5)
+    _native.check(gpu_lib.sb_set_engine(engine - 2 if engine >= 4 else 1))
     _native.check(gpu_lib.sb_set_premac_mode(2 if engine == 3 else 1))
     try:
         for total in (7, 1000, 16384, 16385, 40000):
@@ -368,11 +362,10 @@ def test_minimum_sizes_and_ragged_edges(gpu_lib, engine):
                 assert want[int(i[0])] - want.min() <= 2e-6          # a minimiser (ties on random data are rare)
     finally:
         _native.check(gpu_lib.sb_set_engine(2))
-        _native.check(gpu_lib.sb_set_hop_mode(1))
         _native.check(gpu_lib.sb_set_premac_mode(0))
 
 
-def test_batch_split_into_several_passes(gpu_lib, pair):
+def test_batch_runs_in_several_passes_of_whole_queries(gpu_lib, pair):
     """More template partitions than the resident budget: the batch runs in several passes of whole
     queries and still returns what the single-pass run returns."""
     rs, rd, src, dst = pair['uint8']
@@ -380,13 +373,15 @@ def test_batch_split_into_several_passes(gpu_lib, pair):
     ends = starts + np.tile([0.3, 1.7, 3.2, 4.0], 10)
     centers, windows = starts + 1.0, np.full(40, 10.0)
     want = dst.find_substream_batch(src, starts, ends, centers, windows)
-    _native.check(gpu_lib.sb_set_block_size(8192))
+    # 40 templates of 1 to 4 partitions (B = 16384 samples), at most 7 partition spectra per pass
+    toff, tlen = dst.plan_queries(src, starts, ends, centers, windows)[:2]
+    parts = -(-np.asarray(tlen) // 16384)
+    assert parts.max() <= 7 and parts.sum() > 2 * 7                  # several passes of whole queries
+    _native.check(gpu_lib.sb_set_max_parts(7))
     try:
-        _native.check(gpu_lib.sb_set_max_parts(7))
         got = dst.find_substream_batch(src, starts, ends, centers, windows)
     finally:
         _native.check(gpu_lib.sb_set_max_parts(16384))
-        _native.check(gpu_lib.sb_set_block_size(16384))
     assert np.abs(got[0] - want[0]).max() <= 2e-6 and np.abs(got[1] - want[1]).max() <= SHIFT_TOL
 
 
@@ -422,26 +417,24 @@ def test_values_do_not_depend_on_the_query_range(gpu_lib, pair):
     assert np.array_equal(curves[0], wide[5:1005]) and np.array_equal(curves[1], wide[77777:77777 + 40001])
 
 
-def test_mixed_batch_routes_per_query_and_keeps_caller_order(gpu_lib, pair):
+def test_mixed_batch_of_long_and_short_templates_keeps_caller_order(gpu_lib):
     """A batch mixing short templates (multiply inside the fused kernel) and very long ones (>= 12
     partitions: register-blocked multiply kernel) is processed class by class but returns results in
     the caller's order, and each query's answer equals, bit for bit, its answer when asked alone."""
-    rs, rd, src, dst = pair['uint8']
-    starts = np.array([1.0, 2.0, 3.5, 5.0, 6.0, 8.0, 9.5, 11.0])
-    lens = np.array([0.5, 9.0, 1.0, 10.5, 0.2, 3.0, 12.0, 2.0])        # at B = 8192: 9 / 10.5 / 12 s -> 14 / 16 / 18 partitions
+    from tests.test_gpu_variants import _streams
+    rs, rd, src, dst = _streams(200.0, 17)
+    starts = np.array([10.0, 20.0, 45.0, 60.0, 90.0, 100.0, 120.0, 150.0])
+    lens = np.array([0.5, 17.0, 1.0, 20.0, 0.2, 3.0, 24.0, 2.0])       # 17 / 20 / 24 s -> 13 / 15 / 18 partitions
     ends = starts + lens
     centers, windows = starts + 1.0, np.full(len(starts), 10.0)
-    _native.check(gpu_lib.sb_set_block_size(8192))
-    try:
-        batch = dst.find_substream_batch(src, starts, ends, centers, windows)
-        for q in range(len(starts)):
-            d, t = dst.find_substream(src.get_substream(starts[q], ends[q]), centers[q], windows[q])
-            assert d == batch[0][q] and t == batch[1][q], q
-            d_ref, t_ref = rd.find_substream(rs.get_substream(starts[q], ends[q]), centers[q], windows[q])
-            assert abs(float(d) - float(d_ref)) <= DIFF_TOL and abs(t - t_ref) <= SHIFT_TOL
-        toff, tlen, lag0, nlags, _ = dst.plan_queries(src, starts, ends, centers, windows)
-        curves = dst.match_curves(src, toff, tlen, lag0, nlags)
-        for q in range(len(starts)):
-            assert len(curves[q]) == nlags[q] and curves[q].min() == batch[0][q]
-    finally:
-        _native.check(gpu_lib.sb_set_block_size(16384))
+    batch = dst.find_substream_batch(src, starts, ends, centers, windows)
+    for q in range(len(starts)):
+        d, t = dst.find_substream(src.get_substream(starts[q], ends[q]), centers[q], windows[q])
+        assert d == batch[0][q] and t == batch[1][q], q
+        d_ref, t_ref = rd.find_substream(rs.get_substream(starts[q], ends[q]), centers[q], windows[q])
+        assert abs(float(d) - float(d_ref)) <= DIFF_TOL and abs(t - t_ref) <= SHIFT_TOL
+    toff, tlen, lag0, nlags, _ = dst.plan_queries(src, starts, ends, centers, windows)
+    assert (-(-np.asarray(tlen) // 16384) >= 12).sum() == 3                # three queries take the blocked route
+    curves = dst.match_curves(src, toff, tlen, lag0, nlags)
+    for q in range(len(starts)):
+        assert len(curves[q]) == nlags[q] and curves[q].min() == batch[0][q]

@@ -107,6 +107,9 @@ def test_default_is_the_third_body(gpu_lib):
     assert gpu_lib.sb_set_epilogue(2) != 0 and gpu_lib.sb_get_epilogue() == 3      # the dropped variant is refused
     assert gpu_lib.sb_set_engine(3) != 0 and gpu_lib.sb_set_engine(6) != 0      # dropped engines are refused
     assert gpu_lib.sb_get_engine() == 2
+    # so are the retired cuFFT engine, lag blocks other than 16384 and hop B/2; the settings stay as they were
+    assert gpu_lib.sb_set_engine(0) != 0 and gpu_lib.sb_set_block_size(8192) != 0 and gpu_lib.sb_set_hop_mode(2) != 0
+    assert gpu_lib.sb_get_engine() == 2 and gpu_lib.sb_get_block_size() == 16384
 
 
 @pytest.mark.parametrize('stype', ['uint8', 'float32'])

@@ -19,7 +19,7 @@ for stype in (sys.argv[5].split(',') if len(sys.argv) > 5 else ('uint8', 'float3
     dst = WavStream.from_pcm(dst_pcm, 12000, sample_type=stype)
     starts, ends = synth.make_events(nev, dur, 0, 1.0, 4.0)
     res = {}
-    for eng in ([int(e) for e in sys.argv[6].split(',')] if len(sys.argv) > 6 else (1, 2, 3, 4, 5)):
+    for eng in ([int(e) for e in sys.argv[6].split(',')] if len(sys.argv) > 6 else (1, 2, 4, 5)):
         _native.check(lib.sb_set_engine(eng))
         for r in range(reps):
             d, t = dst.find_substream_batch(src, starts, ends, starts, np.full(len(starts), win))

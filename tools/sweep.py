@@ -31,7 +31,6 @@ ap.add_argument('--queries', type=int, default=512)
 ap.add_argument('--duration', type=float, default=5400.0)
 ap.add_argument('--sample-type', default='uint8')
 ap.add_argument('--reps', type=int, default=3)
-ap.add_argument('--hop-mode', type=int, default=-1)
 ap.add_argument('--premac-mode', type=int, default=-1)
 ap.add_argument('--events', default='0.5,1,3,10,30')
 ap.add_argument('--windows', default='5,10,30,60,120,300,600')
@@ -47,8 +46,6 @@ if a.engine >= 0:
     _native.check(lib.sb_set_engine(a.engine))
 if a.epilogue > 0:
     _native.check(lib.sb_set_epilogue(a.epilogue))
-if a.hop_mode >= 0:
-    _native.check(lib.sb_set_hop_mode(a.hop_mode))
 if a.premac_mode >= 0:
     _native.check(lib.sb_set_premac_mode(a.premac_mode))
 peak = 6650.0
