@@ -39,7 +39,7 @@
 extern "C" {
 #endif
 
-#define SB_ABI_VERSION 4
+#define SB_ABI_VERSION 5
 
 /* status codes */
 #define SB_OK            0
@@ -243,6 +243,16 @@ int sb_flac_index(const void* file, int64_t nbytes, int64_t first_frame_offset, 
                   int framerate, sb_flac** out, int64_t* frames_out);
 int sb_flac_decode(sb_flac* flac, int sample_rate, int64_t padding, int64_t total_len, sb_stream** out_f32);
 int sb_flac_destroy(sb_flac* flac);
+
+/* FLAC frames listed by a container (ABI version 5).  `buf` holds a track's frame payloads back to back (`nbytes`
+ * bytes, no metadata); frame f starts at offsets[f] (increasing) and ends exactly where frame f + 1 starts, the last
+ * at nbytes.  file_offsets[f] is the byte offset in the container file of the block holding frame f: every error
+ * names it.  Each header must parse, agree with the stream parameters and pass its CRC-8 at its listed offset.  The
+ * coded frame / sample numbers are not checked (a cut track starts above 0), and sample positions follow from the
+ * block sizes.  The handle goes to sb_flac_decode and sb_flac_destroy as sb_flac_index's does; the decode then also
+ * requires every frame to end exactly where its lace does. */
+int sb_flac_index_frames(const void* buf, int64_t nbytes, const int64_t* offsets, const int64_t* file_offsets, int64_t n,
+                         int channels, int bits, int framerate, sb_flac** out, int64_t* frames_out);
 
 /* ---- multi-GPU: events shard across ranks (SURVEY.md 8e) ---------------- */
 

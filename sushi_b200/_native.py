@@ -14,7 +14,7 @@ LIB_PATH = os.path.join(_HERE, 'libsushi_b200.so')
 
 SB_OK = 0
 SB_U8, SB_F32 = 0, 1
-ABI_VERSION = 4
+ABI_VERSION = 5
 
 c_i64 = ctypes.c_int64
 c_i64p = ctypes.POINTER(ctypes.c_int64)
@@ -67,6 +67,8 @@ PROTOTYPES = {
     'sb_normalise': (ctypes.c_int, [c_vp, ctypes.c_int, ctypes.POINTER(c_vp), c_f32p, c_f32p]),
     'sb_flac_index': (ctypes.c_int, [c_vp, c_i64, c_i64, ctypes.c_int, ctypes.c_int, ctypes.c_int, ctypes.POINTER(c_vp),
                                      c_i64p]),
+    'sb_flac_index_frames': (ctypes.c_int, [c_vp, c_i64, c_i64p, c_i64p, c_i64, ctypes.c_int, ctypes.c_int, ctypes.c_int,
+                                            ctypes.POINTER(c_vp), c_i64p]),
     'sb_flac_decode': (ctypes.c_int, [c_vp, ctypes.c_int, c_i64, c_i64, ctypes.POINTER(c_vp)]),
     'sb_flac_destroy': (ctypes.c_int, [c_vp]),
     'sb_comm_unique_id': (ctypes.c_int, [c_vp]),

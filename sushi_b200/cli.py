@@ -1,20 +1,28 @@
-"""The Sushi command line for WAV and FLAC inputs: `python -m sushi_b200 --src a.wav --dst b.wav --script s.ass -o out.ass`.
+"""The Sushi command line: `python -m sushi_b200 --src a.mkv --dst b.mkv -o out.ass`.
 
-Flags, defaults and checks are the reference's (sushi.py:528-843).  Demuxing is not supported, so
---src and --dst must be WAV or FLAC files.  For a WAV file the reference starts no subprocess either; a FLAC file
-is decoded on the GPU, where the reference would have ffmpeg convert it (DESIGN.md section 2).  Every
-check runs before the GPU is touched; the run itself is pipeline.shift_script.
+Flags, defaults and checks are the reference's (sushi.py:528-843).  --src and --dst are WAV, FLAC or Matroska
+(.mkv, .mka, .mks, .webm) files.  For a WAV file the reference starts no subprocess either; a FLAC file or a
+Matroska file's FLAC or PCM track is decoded on the GPU, where the reference would have ffmpeg convert it to a WAV
+file (DESIGN.md section 2): no WAV file is ever written.  A Matroska input also gives, as the reference's ffmpeg and
+mkvextract calls do, the script, the chapters and the video timestamps (sushi_b200.matroska); those are written to
+the reference's temporary paths and removed at the end unless --no-cleanup is given.  Every check runs before the GPU
+is touched; the run itself is pipeline.shift_script.
 """
 import argparse
+import io
 import logging
 import os
 import sys
 import time
 
 from . import __version__
+from . import matroska
 from .common import SushiError
 from .pipeline import shift_script
+from .script import format_srt_time
 from .timing import get_ogm_start_times, get_xml_start_times, load_keyframe_times
+
+MATROSKA_EXTENSIONS = ('.mkv', '.mka', '.mks', '.webm')
 
 
 def get_extension(path):
@@ -69,13 +77,13 @@ def create_arg_parser():
     parser.add_argument('--sample-rate', default=12000, type=int, metavar='<rate>', dest='sample_rate',
                         help='Downsampled audio sample rate. [%(default)s]')
 
-    # stream indices select streams of a video; WAV and FLAC inputs have one of each, so they are ignored
+    # stream indices select streams of a Matroska input; WAV and FLAC inputs have one of each, so they are ignored
     parser.add_argument('--src-audio', default=None, type=int, metavar='<id>', dest='src_audio_idx',
-                        help='Audio stream index of the source video (ignored for WAV input)')
+                        help='Audio stream index of the source video (ignored for WAV and FLAC input)')
     parser.add_argument('--src-script', default=None, type=int, metavar='<id>', dest='src_script_idx',
-                        help='Script stream index of the source video (ignored for WAV input)')
+                        help='Script stream index of the source video (ignored for WAV and FLAC input)')
     parser.add_argument('--dst-audio', default=None, type=int, metavar='<id>', dest='dst_audio_idx',
-                        help='Audio stream index of the destination video (ignored for WAV input)')
+                        help='Audio stream index of the destination video (ignored for WAV and FLAC input)')
 
     parser.add_argument('--no-cleanup', action='store_false', dest='cleanup',
                         help="Don't delete demuxed streams")
@@ -100,9 +108,9 @@ def create_arg_parser():
                         help='Timecodes file to use instead of making one from the source (when possible)')
 
     parser.add_argument('--src', required=True, dest='source', metavar='<filename>',
-                        help='Source audio (WAV or FLAC)')
+                        help='Source audio or video (WAV, FLAC or Matroska)')
     parser.add_argument('--dst', required=True, dest='destination', metavar='<filename>',
-                        help='Destination audio (WAV or FLAC)')
+                        help='Destination audio or video (WAV, FLAC or Matroska)')
     parser.add_argument('-o', '--output', default=None, dest='output_script', metavar='<filename>',
                         help='Output script')
 
@@ -112,14 +120,33 @@ def create_arg_parser():
     return parser
 
 
-def _require_wav(path):
-    if get_extension(path) not in ('.wav', '.flac'):
-        raise SushiError('{0}: demuxing is not supported, convert the input to WAV or FLAC first'.format(path))
+def _open_input(path):
+    """None for a WAV or FLAC input; the opened MatroskaFile for a Matroska one.  Anything else, or a Matroska name
+    that does not open as one, is refused where the reference would have ffmpeg demux it."""
+    ext = get_extension(path)
+    if ext in ('.wav', '.flac'):
+        return None
+    if ext in MATROSKA_EXTENSIONS:
+        try:
+            return matroska.MatroskaFile(path)
+        except (OSError, SushiError) as e:
+            raise SushiError('{0}: demuxing is not supported, convert the input to WAV or FLAC first '
+                             '(it does not open as a Matroska file: {1})'.format(path, e))
+    raise SushiError('{0}: demuxing is not supported, convert the input to WAV or FLAC first'.format(path))
+
+
+def _select_audio(mkv, idx):
+    """The stream id of a Matroska input's audio track (None for WAV and FLAC), refusing what cannot be decoded."""
+    if mkv is None:
+        return None
+    track = mkv.select('audio', idx)
+    matroska.audio_codec(track)
+    return track.id
 
 
 def run(args):
-    """sushi.py:528-736 for WAV and FLAC inputs.  Everything up to the shift_script call is validation and
-    small text files; nothing before it touches the GPU."""
+    """sushi.py:528-736.  Everything up to the shift_script call is validation and small text files; nothing before
+    it touches the GPU."""
     ignore_chapters = args.chapters_file is not None and args.chapters_file.lower() == 'none'
 
     check_file_exists(args.source, 'Source')
@@ -138,10 +165,48 @@ def run(args):
         raise SushiError('Both fps and timecodes file cannot be specified at the same time')
 
     # where the reference opens the inputs with ffmpeg (sushi.py:553-554)
-    _require_wav(args.source)
-    _require_wav(args.destination)
+    src_mkv = _open_input(args.source)
+    try:
+        dst_mkv = _open_input(args.destination)
+    except SushiError:
+        if src_mkv:
+            src_mkv.close()
+        raise
+    written = []
+    try:
+        return _run(args, ignore_chapters, src_mkv, dst_mkv, written)
+    finally:
+        for m in (src_mkv, dst_mkv):
+            if m:
+                m.close()
+        if args.cleanup:
+            for path in written:
+                if os.path.exists(path):
+                    os.remove(path)
 
-    if not args.script_file:
+
+def _run(args, ignore_chapters, src_mkv, dst_mkv, written):
+    src_track = _select_audio(src_mkv, args.src_audio_idx)
+    dst_track = _select_audio(dst_mkv, args.dst_audio_idx)
+    # files taken out of the inputs, written once every check has passed: (path, function giving the text); and per
+    # Matroska input, the tracks one walk over its clusters reads: (frames read, block times only)
+    extract = []
+    walks = [(m, [t], []) for m, t in ((src_mkv, src_track), (dst_mkv, dst_track)) if m is not None]
+
+    def read_with_audio(mkv, payload=None, times=None):
+        for m, p, t in walks:
+            if m is mkv:
+                p += [payload] if payload is not None else []
+                t += [times] if times is not None else []
+
+    if args.script_file:
+        src_script_path = args.script_file
+    elif src_mkv is not None:
+        script_track = src_mkv.select('subtitles', args.src_script_idx)
+        src_script_path = format_full_path(args.temp_dir, args.source, '.sushi' + script_track.script_type)
+        extract.append((src_script_path, lambda: src_mkv.script_text(script_track)))
+        read_with_audio(src_mkv, payload=script_track.id)
+    else:
         raise SushiError("Script file isn't specified")
 
     if (args.src_keyframes and not args.dst_keyframes) or (args.dst_keyframes and not args.src_keyframes):
@@ -149,7 +214,6 @@ def run(args):
 
     create_directory_if_not_exists(args.temp_dir)
 
-    src_script_path = args.script_file
     script_extension = get_extension(src_script_path)
     if script_extension not in ('.ass', '.srt'):
         raise SushiError('Unknown script type')
@@ -163,43 +227,73 @@ def run(args):
     else:
         dst_script_path = format_full_path(args.temp_dir, args.destination, '.sushi' + script_extension)
 
-    # a WAV input carries no chapters of its own
     if args.grouping and not ignore_chapters and args.chapters_file:
         if get_extension(args.chapters_file) == '.xml':
             chapter_times = get_xml_start_times(args.chapters_file)
         else:
             chapter_times = get_ogm_start_times(args.chapters_file)
+    elif args.grouping and not ignore_chapters and src_mkv is not None:
+        # the source's own chapters, also written out as OGM as the reference does (chapters.py:35-37)
+        chapter_times = src_mkv.chapters
+        extract.append((format_full_path(args.temp_dir, args.source, '.sushi.chapters.txt'), lambda: ''.join(
+            'CHAPTER{0:02}={1}\nCHAPTER{0:02}NAME=\n'.format(i + 1, format_srt_time(t).replace(',', '.'))
+            for i, t in enumerate(chapter_times))))
     else:
         chapter_times = []
 
     keyframes = None
     if args.src_keyframes:
-        def select_keyframes(file_arg, path):
+        def select_keyframes(file_arg, path, mkv):
             if file_arg in ('auto', 'make'):
                 auto_file = format_full_path(args.temp_dir, path, '.sushi.keyframes.txt')
                 if file_arg == 'make' or not os.path.exists(auto_file):
-                    raise SushiError("Cannot make keyframes for {0} because it doesn't have any video!".format(path))
+                    if mkv is None or not mkv.streams('video'):
+                        raise SushiError("Cannot make keyframes for {0} because it doesn't have any video!".format(path))
+                    raise SushiError('Cannot make keyframes for {0}: making keyframes (SCXvid) is not supported, '
+                                     'pass a keyframes file'.format(path))
                 return auto_file
             return file_arg
 
-        def select_timecodes(external_file, fps_arg):
-            if external_file or fps_arg:
+        def select_timecodes(external_file, fps_arg, path, mkv):
+            if external_file:
                 return external_file
+            if fps_arg:
+                return None
+            if mkv is not None and mkv.streams('video'):
+                out = format_full_path(args.temp_dir, path, '.sushi.timecodes.txt')
+                extract.append((out, mkv.timecodes_text))
+                read_with_audio(mkv, times=mkv.streams('video')[0].id)
+                return out
             raise SushiError('Fps, timecodes or video files must be provided if keyframes are used')
 
-        src_keyframes_file = select_keyframes(args.src_keyframes, args.source)
-        dst_keyframes_file = select_keyframes(args.dst_keyframes, args.destination)
-        src_timecodes_file = select_timecodes(args.src_timecodes, args.src_fps)
-        dst_timecodes_file = select_timecodes(args.dst_timecodes, args.dst_fps)
+        src_keyframes_file = select_keyframes(args.src_keyframes, args.source, src_mkv)
+        dst_keyframes_file = select_keyframes(args.dst_keyframes, args.destination, dst_mkv)
+        src_timecodes_file = select_timecodes(args.src_timecodes, args.src_fps, args.source, src_mkv)
+        dst_timecodes_file = select_timecodes(args.dst_timecodes, args.dst_fps, args.destination, dst_mkv)
+
+    # every check has passed: one walk per Matroska input reads its audio, script and video times; the side products
+    # are written from it, and the audio stays in memory for WavStream
+    for mkv, payload_ids, time_ids in walks:
+        mkv.prefetch(payload_ids, time_ids)
+    for path, make in extract:
+        text = make()
+        written.append(path)
+        with io.open(path, 'w', encoding='utf-8', newline='') as f:
+            f.write(text)
+
+    if args.src_keyframes:
         keyframes = load_keyframe_times(src_keyframes_file, dst_keyframes_file, args.src_fps, args.dst_fps,
                                         src_timecodes_file, dst_timecodes_file)
 
-    return shift_script(args.source, args.destination, src_script_path, dst_script_path,
+    tracks = {} if src_track is None and dst_track is None else dict(src_track=src_track, dst_track=dst_track)
+    src = args.source if src_mkv is None else src_mkv
+    dst = args.destination if dst_mkv is None else dst_mkv
+    return shift_script(src, dst, src_script_path, dst_script_path,
                         sample_rate=args.sample_rate, sample_type=args.sample_type, chapter_times=chapter_times,
                         window=args.window, max_window=args.max_window, rewind_thresh=args.rewind_thresh,
                         grouping=args.grouping, smooth_radius=args.smooth_radius,
                         max_ts_duration=args.max_ts_duration, max_ts_distance=args.max_ts_distance,
-                        keyframes=keyframes, max_kf_distance=args.max_kf_distance, kf_mode=args.kf_mode)
+                        keyframes=keyframes, max_kf_distance=args.max_kf_distance, kf_mode=args.kf_mode, **tracks)
 
 
 def main(argv=None):

@@ -3,6 +3,9 @@
 //   sb_flac_index   upload the file; k_flac_sync lists every byte position holding a sync code and a frame header
 //                   that parses, agrees with STREAMINFO and passes its CRC-8 (false syncs included); the host chains
 //                   the real frames from the first one by their coded frame / sample numbers
+//   sb_flac_index_frames  the same for frames a container lists (Matroska blocks and laces): k_flac_frames, one thread
+//                   per listed frame, checks the header at its offset; sample positions are the prefix sum of the
+//                   block sizes, and errors name the file offset of the frame's block
 //   sb_flac_decode  k_flac_decode: one thread per frame decodes its subframes in turn (a subframe starts where the
 //                   previous one ends) and checks the frame's CRC-16 and end; k_flac_decorrelate: one CTA per frame
 //                   undoes the stereo decorrelation and writes int16 (24-bit: the top 16 bits); then the loader
@@ -43,6 +46,14 @@ k_flac_sync(const uint8_t* __restrict__ file, int64_t first, int64_t nbytes, int
     }
 }
 
+// Frames listed by a container: one thread per frame parses the header at its listed offset, bounded by the next one
+__global__ void __launch_bounds__(256)
+k_flac_frames(const uint8_t* __restrict__ buf, int64_t nbytes, const int64_t* __restrict__ offsets, int64_t n,
+              int channels, int bits, int rate, sbflac::ListedFrame* __restrict__ out) {
+    const int64_t f = (int64_t)blockIdx.x * blockDim.x + threadIdx.x;
+    if (f < n) out[f] = sbflac::listed_frame(buf, nbytes, offsets, n, f, channels, bits, rate);
+}
+
 __global__ void __launch_bounds__(64)
 k_flac_decode(const uint8_t* __restrict__ file, const FrameDesc* __restrict__ frames, int64_t n_frames, int channels,
               int bits, int rate, int32_t* __restrict__ planar, sbflac::FrameStatus* __restrict__ status) {
@@ -77,6 +88,7 @@ struct sb_flac {
     int64_t nbytes = 0;
     int channels = 0, bits = 0, framerate = 0;
     std::vector<FrameDesc> frames;
+    std::vector<int64_t> where;        // sb_flac_index_frames: file offset of each frame's block (messages name it)
     int64_t samples = 0;
 };
 
@@ -144,6 +156,56 @@ int sb_flac_index(const void* file, int64_t nbytes, int64_t first_frame_offset, 
     return SB_OK;
 }
 
+int sb_flac_index_frames(const void* buf, int64_t nbytes, const int64_t* offsets, const int64_t* file_offsets, int64_t n,
+                         int channels, int bits, int framerate, sb_flac** out, int64_t* frames_out) {
+    Ctx& c = ctx();
+    if (!c.inited) SB_FAIL(SB_ESTATE, "sb_flac_index_frames: library not initialised (call sb_init)");
+    if (!buf || !offsets || !file_offsets || !out || !frames_out) SB_FAIL(SB_EINVAL, "sb_flac_index_frames: NULL argument");
+    if (bits != 16 && bits != 24) SB_FAIL(SB_EINVAL, "FLAC with %d bits per sample is not supported (16 or 24)", bits);
+    if (channels < 1 || channels > 8 || framerate < 1 || nbytes < 1 || n < 0)
+        SB_FAIL(SB_EINVAL, "sb_flac_index_frames: bad stream parameters");
+    for (int64_t f = 0; f < n; ++f)
+        if (offsets[f] < 0 || offsets[f] >= nbytes || (f > 0 && offsets[f] <= offsets[f - 1]))
+            SB_FAIL(SB_EINVAL, "FLAC frame %lld at byte offset %lld: %s", (long long)f, (long long)file_offsets[f],
+                    offsets[f] < 0 || offsets[f] >= nbytes ? "frame starts outside the buffer" : "empty frame");
+    sb_flac* h = new (std::nothrow) sb_flac();
+    if (!h) SB_FAIL(SB_ENOMEM, "sb_flac_index_frames: out of host memory");
+    h->nbytes = nbytes; h->channels = channels; h->bits = bits; h->framerate = framerate;
+    h->where.assign(file_offsets, file_offsets + n);
+    auto fail = [&](int code) { sb_flac_destroy(h); return code; };
+    if (pool_alloc((void**)&h->d_file, (size_t)nbytes + 16) != SB_OK) return fail(SB_ENOMEM);
+    int64_t* d_offsets = nullptr;
+    sbflac::ListedFrame* d_listed = nullptr;
+    if (pool_alloc((void**)&d_offsets, sizeof(int64_t) * n + 16) != SB_OK) return fail(SB_ENOMEM);
+    if (pool_alloc((void**)&d_listed, sizeof(sbflac::ListedFrame) * n + 16) != SB_OK) { pool_free(d_offsets); return fail(SB_ENOMEM); }
+    std::vector<sbflac::ListedFrame> listed((size_t)n);
+    cudaError_t e = cudaMemsetAsync(h->d_file + (nbytes & ~(int64_t)3), 0, 16, c.stream);
+    if (e == cudaSuccess) e = cudaMemcpyAsync(h->d_file, buf, (size_t)nbytes, cudaMemcpyHostToDevice, c.stream);
+    if (e == cudaSuccess) e = cudaMemcpyAsync(d_offsets, offsets, sizeof(int64_t) * n, cudaMemcpyHostToDevice, c.stream);
+    if (e == cudaSuccess && n > 0) {
+        ProfScope ps("flac_frames");
+        k_flac_frames<<<(unsigned)((n + 255) / 256), 256, 0, c.stream>>>(h->d_file, nbytes, d_offsets, n, channels, bits,
+                                                                         framerate, d_listed);
+        e = cudaGetLastError();
+    }
+    if (e == cudaSuccess) e = cudaMemcpyAsync(listed.data(), d_listed, sizeof(sbflac::ListedFrame) * n,
+                                              cudaMemcpyDeviceToHost, c.stream);
+    if (e == cudaSuccess) e = cudaStreamSynchronize(c.stream);
+    pool_free(d_offsets); pool_free(d_listed);
+    if (e != cudaSuccess) { sb_flac_destroy(h); SB_FAIL(SB_ECUDA, "sb_flac_index_frames: %s", cudaGetErrorString(e)); }
+    char msg[256];
+    int64_t sample = 0;
+    if (!sbflac::list_frames(listed.data(), offsets, file_offsets, n, nbytes, h->frames, &sample, msg, sizeof(msg))) {
+        sb::set_error("%s", msg);
+        sb_flac_destroy(h);
+        return SB_EINVAL;
+    }
+    h->samples = sample;
+    *frames_out = sample;
+    *out = h;
+    return SB_OK;
+}
+
 int sb_flac_decode(sb_flac* h, int sample_rate, int64_t padding, int64_t total_len, sb_stream** out_f32) {
     Ctx& c = ctx();
     if (!c.inited) SB_FAIL(SB_ESTATE, "sb_flac_decode: library not initialised (call sb_init)");
@@ -177,7 +239,8 @@ int sb_flac_decode(sb_flac* h, int sample_rate, int64_t padding, int64_t total_l
     auto bytes_at = [&](int64_t off, uint8_t* buf) {
         if (off < h->nbytes) cudaMemcpy(buf, h->d_file + off, (size_t)std::min<int64_t>(16, h->nbytes - off), cudaMemcpyDeviceToHost);
     };
-    if (!sbflac::check_frames(h->frames, status.data(), h->nbytes, ch, h->bits, h->framerate, bytes_at, msg, sizeof(msg))) {
+    if (!sbflac::check_frames(h->frames, status.data(), h->nbytes, ch, h->bits, h->framerate, bytes_at, msg, sizeof(msg),
+                              h->where.empty() ? nullptr : h->where.data())) {
         release();
         SB_FAIL(SB_EINVAL, "%s", msg);
     }

@@ -395,16 +395,67 @@ inline bool chain(std::vector<Candidate>& cand, int64_t first_offset, int64_t nb
     return true;
 }
 
+// ---- frames listed by a container (host and k_flac_frames) -------------------------------------------------------
+// In a Matroska track the frame boundaries are the block and lace boundaries: frame f occupies [offsets[f], limit),
+// limit being the next listed offset (the buffer size for the last).  What one frame's header says, or why it is
+// refused: the header must parse, agree with STREAMINFO and pass its CRC-8 right at its offset
+struct ListedFrame { int32_t code; int32_t block_size; int32_t assignment; int32_t pad; };
+
+SBF_HD ListedFrame listed_frame(const uint8_t* buf, int64_t nbytes, const int64_t* offsets, int64_t n, int64_t f,
+                                int channels, int bits, int rate) {
+    ListedFrame r; r.code = kOk; r.block_size = 0; r.assignment = 0; r.pad = 0;
+    const int64_t off = offsets[f], limit = f + 1 < n ? offsets[f + 1] : nbytes;
+    if (off < 0 || limit > nbytes || limit < off) { r.code = kTruncated; return r; }
+    Header h;
+    const int rc = parse_header(buf + off, limit - off, channels, bits, rate, &h);
+    if (rc != kOk) { r.code = rc == kBadSync && limit - off < 16 ? kTruncated : rc; return r; }
+    r.block_size = h.block_size; r.assignment = h.assignment;
+    return r;
+}
+
+// The frame table of listed frames: sample positions are the prefix sum of the header block sizes (a track cut from a
+// longer stream starts at a coded number above 0, so the numbers are not required to run on).  `where` names each
+// frame's block by its file offset in the message.  Returns false with a message.
+inline bool list_frames(const ListedFrame* listed, const int64_t* offsets, const int64_t* where, int64_t n, int64_t nbytes,
+                        std::vector<FrameDesc>& frames, int64_t* samples, char* msg, size_t msg_len) {
+    frames.clear();
+    int64_t sample = 0;
+    for (int64_t f = 0; f < n; ++f) {
+        if (listed[f].code != kOk) {
+            snprintf(msg, msg_len, "FLAC frame %lld at byte offset %lld: %s", (long long)f, (long long)where[f],
+                     error_text(listed[f].code));
+            return false;
+        }
+        FrameDesc d;
+        d.offset = offsets[f]; d.limit = f + 1 < n ? offsets[f + 1] : nbytes; d.sample = sample;
+        d.block_size = listed[f].block_size; d.assignment = listed[f].assignment;
+        frames.push_back(d);
+        sample += listed[f].block_size;
+    }
+    *samples = sample;
+    return true;
+}
+
 // Every frame must have decoded, passed its CRC-16 and ended exactly at its limit.  bytes_at(offset, buf16) fetches
-// the (at most 16) bytes at an offset for the message about a missing frame.  Returns false with a message.
+// the (at most 16) bytes at an offset for the message about a missing frame.  `where` (NULL for a FLAC file) gives
+// the file offset of each listed frame's block: messages then name it, and a frame must end exactly where its lace
+// does.  Returns false with a message.
 template <class BytesAt>
 bool check_frames(const std::vector<FrameDesc>& frames, const FrameStatus* status, int64_t nbytes, int channels, int bits,
-                  int rate, BytesAt bytes_at, char* msg, size_t msg_len) {
+                  int rate, BytesAt bytes_at, char* msg, size_t msg_len, const int64_t* where = nullptr) {
     const int64_t nf = (int64_t)frames.size();
     for (int64_t f = 0; f < nf; ++f) {
         const FrameDesc& d = frames[f];
         const FrameStatus& st = status[f];
         const bool last = f == nf - 1;
+        if (where) {
+            if (st.code != kOk || st.end != d.limit) {
+                snprintf(msg, msg_len, "FLAC frame %lld at byte offset %lld: %s", (long long)f, (long long)where[f],
+                         st.code != kOk ? error_text(st.code) : "frame does not end where its lace ends");
+                return false;
+            }
+            continue;
+        }
         if (st.code != kOk) {
             snprintf(msg, msg_len, "FLAC frame %lld at byte offset %lld: %s", (long long)f, (long long)d.offset,
                      error_text(st.code == kOverrun && last ? kTruncated : st.code));

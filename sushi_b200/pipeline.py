@@ -94,13 +94,15 @@ def _resolve_links(events):
 
 
 def shift_script(src_audio, dst_audio, script_path, output_path, sample_rate=12000, sample_type='uint8',
-                 chapter_times=(), **options):
-    """src/dst WAV or FLAC + ASS/SRT script in, shifted script out (the audio-in/script-out core of the CLI).
+                 chapter_times=(), src_track=None, dst_track=None, **options):
+    """src/dst WAV, FLAC or Matroska (a path, or an opened MatroskaFile) + ASS/SRT script in, shifted script out (the
+    audio-in/script-out core of the CLI).
+    src_track / dst_track are the audio stream ids of Matroska inputs (None: the reference's default rule).
     `options` are shift_events' keyword arguments, keyframes included."""
     script = load_script(script_path)
     script.sort_by_time()
-    src = WavStream(src_audio, sample_rate=sample_rate, sample_type=sample_type)
-    dst = WavStream(dst_audio, sample_rate=sample_rate, sample_type=sample_type)
+    src = WavStream(src_audio, sample_rate=sample_rate, sample_type=sample_type, track=src_track)
+    dst = WavStream(dst_audio, sample_rate=sample_rate, sample_type=sample_type, track=dst_track)
     groups = shift_events(script.events, src, dst, chapter_times=chapter_times, **options)
     for e in script.events:
         e.apply_shift()

@@ -14,6 +14,7 @@ sample conversions stay here, in Python, written exactly as the reference writes
 them, so the integer offsets handed to the library are bit-identical.
 """
 import ctypes
+import io
 import logging
 import math
 import os
@@ -23,7 +24,7 @@ from time import time
 
 import numpy as np
 
-from . import _native
+from . import _native, matroska
 from ._nvtx import nvtx_range
 from .common import SushiError, clip, py2_round
 
@@ -150,7 +151,18 @@ class FlacFile(object):
     def __init__(self, path):
         with open(path, 'rb') as f:
             self.data = f.read()
-        d = self.data
+        self._parse(self.data, path)
+
+    @classmethod
+    def from_bytes(cls, data, name):
+        """The metadata of `data` (a Matroska track's CodecPrivate: the marker and the metadata blocks, no frames);
+        messages name `name`."""
+        self = object.__new__(cls)
+        self.data = bytes(data)
+        self._parse(self.data, name)
+        return self
+
+    def _parse(self, d, path):
         at = id3v2_size(d[:10])
         if d[at:at + 4] != FLAC_MAGIC:
             raise SushiError('{0}: not a FLAC file'.format(path))
@@ -300,14 +312,20 @@ class StreamGeometry(object):
 class WavStream(StreamGeometry):
     READ_CHUNK_SIZE = 1  # seconds per resample chunk (wav.py:105)
 
-    def __init__(self, path, sample_rate=12000, sample_type='uint8', device=None, loader='gpu'):
+    def __init__(self, path, sample_rate=12000, sample_type='uint8', device=None, loader='gpu', track=None):
         """loader='gpu' (default): decode / resample / pad / normalise on the GPU (sb_load_pcm +
         sb_normalise); loader='host' runs the NumPy mirror of the same arithmetic and uploads the
-        result (kept as the cross-check; both give bit-identical .data)."""
+        result (kept as the cross-check; both give bit-identical .data).  A Matroska file loads its audio track
+        `track` (a stream id; None: the only audio track, else the default one, as the reference selects); `path` may
+        also be an opened MatroskaFile, whose frames then come from one walk shared with the script and timecodes."""
         if sample_type not in _DTYPES:
             raise SushiError('Unknown sample type of WAV stream, must be uint8 or float32')
         self._handle = None
         before_read = time()
+        if isinstance(path, matroska.MatroskaFile) or matroska.is_matroska(path):
+            self._load_matroska(path, sample_rate, sample_type, device, loader, track)
+            logging.info('Done reading Matroska {0} in {1}s'.format(path, time() - before_read))
+            return
         if is_flac(path):
             self._load_flac(path, sample_rate, sample_type, device, loader)
             logging.info('Done reading FLAC {0} in {1}s'.format(path, time() - before_read))
@@ -361,6 +379,68 @@ class WavStream(StreamGeometry):
                         path, flac.total_samples, frames.value))
                 return raw
             self._load_gpu_with(decode, frames.value, flac.framerate, sample_rate, sample_type, device)
+        finally:
+            lib.sb_flac_destroy(h)
+
+    def _load_matroska(self, path, sample_rate, sample_type, device, loader, track):
+        """A Matroska audio track loads exactly as the plain PCM WAV of its decoded samples, frames concatenated in
+        block order (timestamp gaps are not filled).  FLAC frames are decoded on the GPU where the container lists
+        them (sb_flac_index_frames; a cut track's frame numbers and stale STREAMINFO total are not checked);
+        little-endian PCM is a WAV data chunk as it stands and goes through sb_load_pcm.  `path` is a file name or an
+        opened MatroskaFile (left open; the track's table is released from it)."""
+        opened = isinstance(path, matroska.MatroskaFile)
+        mkv = path if opened else matroska.MatroskaFile(path)
+        path = mkv.path
+        try:
+            t = mkv.select('audio', track)
+            kind = matroska.audio_codec(t)
+            if kind == 'flac':
+                info = FlacFile.from_bytes(t.codec_private, '{0} track {1}'.format(path, t.id))
+                if info.bits_per_sample not in (16, 24):
+                    raise SushiError('FLAC with {0} bits per sample is not supported (16 or 24)'.format(
+                        info.bits_per_sample))
+                if loader != 'gpu':
+                    raise SushiError("{0}: FLAC input needs loader='gpu' (there is no host FLAC decoder)".format(path))
+            table = mkv.frames([t.id])[t.id]
+            mkv.release([t.id])
+        finally:
+            if not opened:
+                mkv.close()
+        if kind == 'flac':
+            table.refuse_empty(path, 'FLAC')
+        if kind == 'pcm':
+            width = t.bit_depth // 8
+            frames = len(table.data) // (t.channels * width)
+            rate = int(t.sampling_frequency)
+            if loader == 'gpu':
+                self._load_gpu(table.data, frames, t.channels, width, rate, sample_rate, sample_type, device)
+            else:
+                mem = DownmixedWavFile.__new__(DownmixedWavFile)
+                mem._file = io.BytesIO(table.data)
+                mem.channels_count, mem.framerate, mem.sample_width = t.channels, rate, width
+                mem.frame_size, mem.frames_count = t.channels * width, frames
+                self._load(mem, sample_rate, sample_type)
+                self._upload(device)
+            return
+        lib = _native.lib(device)
+        h = ctypes.c_void_p()
+        n = ctypes.c_int64()
+        buf = np.frombuffer(table.data + b'\0', dtype=np.uint8)          # never empty
+        offsets = np.ascontiguousarray(table.offset, np.int64)
+        blocks = np.ascontiguousarray(table.block, np.int64)
+        with nvtx_range('sushi_b200: sb_flac_index_frames'):
+            _native.check(lib.sb_flac_index_frames(buf.ctypes.data_as(ctypes.c_void_p), len(table.data) or 1,
+                                                   offsets.ctypes.data_as(_native.c_i64p),
+                                                   blocks.ctypes.data_as(_native.c_i64p), len(offsets),
+                                                   info.channels_count, info.bits_per_sample, info.framerate,
+                                                   ctypes.byref(h), ctypes.byref(n)), 'sb_flac_index_frames')
+        try:
+            def decode(padding, total):
+                raw = ctypes.c_void_p()
+                with nvtx_range('sushi_b200: sb_flac_decode'):
+                    _native.check(lib.sb_flac_decode(h, sample_rate, padding, total, ctypes.byref(raw)), 'sb_flac_decode')
+                return raw
+            self._load_gpu_with(decode, n.value, info.framerate, sample_rate, sample_type, device)
         finally:
             lib.sb_flac_destroy(h)
 
