@@ -39,7 +39,7 @@
 extern "C" {
 #endif
 
-#define SB_ABI_VERSION 5
+#define SB_ABI_VERSION 6
 
 /* status codes */
 #define SB_OK            0
@@ -54,6 +54,7 @@ extern "C" {
 
 typedef struct sb_stream sb_stream;      /* opaque: one normalised stream in HBM */
 typedef struct sb_flac sb_flac;          /* opaque: an indexed FLAC file on the device */
+typedef struct sb_truehd sb_truehd;      /* opaque: a decoded TrueHD stream on the device */
 
 /* ---- life cycle ------------------------------------------------------- */
 
@@ -253,6 +254,26 @@ int sb_flac_destroy(sb_flac* flac);
  * requires every frame to end exactly where its lace does. */
 int sb_flac_index_frames(const void* buf, int64_t nbytes, const int64_t* offsets, const int64_t* file_offsets, int64_t n,
                          int channels, int bits, int framerate, sb_flac** out, int64_t* frames_out);
+
+/* ---- Dolby TrueHD input (ABI version 6) ---------------------------------------
+ *
+ * A TrueHD stream loads exactly as the plain PCM WAV of the samples FFmpeg's decoder returns loads through
+ * sb_load_pcm: the top 16 bits of each 24-bit sample, channels in FFmpeg's order, the presentation of substream
+ * min(n - 1, 2) (a fourth, object substream is skipped).  `buf` holds the stream's bytes (`nbytes`); a container's
+ * blocks start at offsets[0..n) (increasing, back to back; a raw .thd stream is one block at 0) and
+ * file_offsets[b] is the byte offset in the file of block b, which errors name (a negative one: errors name the
+ * AU's own offset, as for a raw stream).  An access unit (AU) must end inside its block.
+ * sb_truehd_index uploads the stream, lists its major syncs on the GPU, chains the AUs into restart segments on the
+ * host and decodes every segment on the GPU, one thread each.  It fails with SB_EINVAL, sb_last_error() naming the
+ * AU index and byte offset, on any damage listed in DESIGN.md section 2: check nibble, major sync CRC, restart header
+ * checksum, substream parity or CRC, lossless check, AU lengths, a segment without restart headers, a short AU
+ * before the end.  MLP is refused.  info[0..1] receive the channel count and the sample rate; *frames_out the
+ * decoded samples per channel.
+ * sb_truehd_decode resamples to sample_rate and pads exactly as sb_load_pcm does, into a SB_F32 stream. */
+int sb_truehd_index(const void* buf, int64_t nbytes, const int64_t* offsets, const int64_t* file_offsets, int64_t n,
+                    int32_t* info, sb_truehd** out, int64_t* frames_out);
+int sb_truehd_decode(sb_truehd* thd, int sample_rate, int64_t padding, int64_t total_len, sb_stream** out_f32);
+int sb_truehd_destroy(sb_truehd* thd);
 
 /* ---- multi-GPU: events shard across ranks (SURVEY.md 8e) ---------------- */
 

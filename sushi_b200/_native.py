@@ -14,7 +14,7 @@ LIB_PATH = os.path.join(_HERE, 'libsushi_b200.so')
 
 SB_OK = 0
 SB_U8, SB_F32 = 0, 1
-ABI_VERSION = 5
+ABI_VERSION = 6
 
 c_i64 = ctypes.c_int64
 c_i64p = ctypes.POINTER(ctypes.c_int64)
@@ -71,6 +71,9 @@ PROTOTYPES = {
                                             ctypes.POINTER(c_vp), c_i64p]),
     'sb_flac_decode': (ctypes.c_int, [c_vp, ctypes.c_int, c_i64, c_i64, ctypes.POINTER(c_vp)]),
     'sb_flac_destroy': (ctypes.c_int, [c_vp]),
+    'sb_truehd_index': (ctypes.c_int, [c_vp, c_i64, c_i64p, c_i64p, c_i64, c_i32p, ctypes.POINTER(c_vp), c_i64p]),
+    'sb_truehd_decode': (ctypes.c_int, [c_vp, ctypes.c_int, c_i64, c_i64, ctypes.POINTER(c_vp)]),
+    'sb_truehd_destroy': (ctypes.c_int, [c_vp]),
     'sb_comm_unique_id': (ctypes.c_int, [c_vp]),
     'sb_comm_init': (ctypes.c_int, [c_vp, ctypes.c_int, ctypes.c_int]),
     'sb_comm_destroy': (ctypes.c_int, []),

@@ -108,9 +108,9 @@ def create_arg_parser():
                         help='Timecodes file to use instead of making one from the source (when possible)')
 
     parser.add_argument('--src', required=True, dest='source', metavar='<filename>',
-                        help='Source audio or video (WAV, FLAC or Matroska)')
+                        help='Source audio or video (WAV, FLAC, TrueHD or Matroska)')
     parser.add_argument('--dst', required=True, dest='destination', metavar='<filename>',
-                        help='Destination audio or video (WAV, FLAC or Matroska)')
+                        help='Destination audio or video (WAV, FLAC, TrueHD or Matroska)')
     parser.add_argument('-o', '--output', default=None, dest='output_script', metavar='<filename>',
                         help='Output script')
 
@@ -121,10 +121,10 @@ def create_arg_parser():
 
 
 def _open_input(path):
-    """None for a WAV or FLAC input; the opened MatroskaFile for a Matroska one.  Anything else, or a Matroska name
+    """None for a WAV, FLAC or raw TrueHD (.thd) input; the opened MatroskaFile for a Matroska one.  Anything else, or a Matroska name
     that does not open as one, is refused where the reference would have ffmpeg demux it."""
     ext = get_extension(path)
-    if ext in ('.wav', '.flac'):
+    if ext in ('.wav', '.flac', '.thd'):
         return None
     if ext in MATROSKA_EXTENSIONS:
         try:

@@ -24,7 +24,7 @@ from time import time
 
 import numpy as np
 
-from . import _native, matroska
+from . import _native, matroska, truehd
 from ._nvtx import nvtx_range
 from .common import SushiError, clip, py2_round
 
@@ -326,6 +326,10 @@ class WavStream(StreamGeometry):
             self._load_matroska(path, sample_rate, sample_type, device, loader, track)
             logging.info('Done reading Matroska {0} in {1}s'.format(path, time() - before_read))
             return
+        if truehd.is_truehd(path):
+            self._load_truehd(path, sample_rate, sample_type, device, loader)
+            logging.info('Done reading TrueHD {0} in {1}s'.format(path, time() - before_read))
+            return
         if is_flac(path):
             self._load_flac(path, sample_rate, sample_type, device, loader)
             logging.info('Done reading FLAC {0} in {1}s'.format(path, time() - before_read))
@@ -382,6 +386,40 @@ class WavStream(StreamGeometry):
         finally:
             lib.sb_flac_destroy(h)
 
+    def _load_truehd(self, path, sample_rate, sample_type, device, loader):
+        """A raw TrueHD stream loads exactly as the plain PCM WAV of the samples FFmpeg's decoder returns (their top 16
+        bits): one block holding every access unit, decoded on the GPU.  There is no host decoder."""
+        data, _ = truehd.read_stream(path)
+        if loader != 'gpu':
+            raise SushiError("{0}: TrueHD input needs loader='gpu' (there is no host TrueHD decoder)".format(path))
+        # one block; a negative file offset makes messages name each access unit's own offset
+        self._load_truehd_blocks(data, np.zeros(1, np.int64), np.full(1, -1, np.int64), sample_rate, sample_type, device)
+
+    def _load_truehd_blocks(self, data, offsets, blocks, sample_rate, sample_type, device):
+        """sb_truehd_index on the stream's blocks (offsets into data; blocks: their file offsets), then the loader."""
+        lib = _native.lib(device)
+        h = ctypes.c_void_p()
+        n = ctypes.c_int64()
+        info = np.zeros(2, np.int32)
+        buf = np.frombuffer(data + b'\0', dtype=np.uint8)
+        offsets = np.ascontiguousarray(offsets, np.int64)
+        blocks = np.ascontiguousarray(blocks, np.int64)
+        with nvtx_range('sushi_b200: sb_truehd_index'):
+            _native.check(lib.sb_truehd_index(buf.ctypes.data_as(ctypes.c_void_p), len(data),
+                                              offsets.ctypes.data_as(_native.c_i64p), blocks.ctypes.data_as(_native.c_i64p),
+                                              len(offsets), info.ctypes.data_as(_native.c_i32p), ctypes.byref(h),
+                                              ctypes.byref(n)), 'sb_truehd_index')
+        try:
+            def decode(padding, total):
+                raw = ctypes.c_void_p()
+                with nvtx_range('sushi_b200: sb_truehd_decode'):
+                    _native.check(lib.sb_truehd_decode(h, sample_rate, padding, total, ctypes.byref(raw)),
+                                  'sb_truehd_decode')
+                return raw
+            self._load_gpu_with(decode, n.value, int(info[1]), sample_rate, sample_type, device)
+        finally:
+            lib.sb_truehd_destroy(h)
+
     def _load_matroska(self, path, sample_rate, sample_type, device, loader, track):
         """A Matroska audio track loads exactly as the plain PCM WAV of its decoded samples, frames concatenated in
         block order (timestamp gaps are not filled).  FLAC frames are decoded on the GPU where the container lists
@@ -401,6 +439,8 @@ class WavStream(StreamGeometry):
                         info.bits_per_sample))
                 if loader != 'gpu':
                     raise SushiError("{0}: FLAC input needs loader='gpu' (there is no host FLAC decoder)".format(path))
+            if kind == 'truehd' and loader != 'gpu':
+                raise SushiError("{0}: TrueHD input needs loader='gpu' (there is no host TrueHD decoder)".format(path))
             table = mkv.frames([t.id])[t.id]
             mkv.release([t.id])
         finally:
@@ -408,6 +448,11 @@ class WavStream(StreamGeometry):
                 mkv.close()
         if kind == 'flac':
             table.refuse_empty(path, 'FLAC')
+        if kind == 'truehd':
+            table.refuse_empty(path, 'TrueHD')
+            truehd.MajorSync(table.data[:64], '{0} track {1}'.format(path, t.id))
+            self._load_truehd_blocks(table.data, table.offset, table.block, sample_rate, sample_type, device)
+            return
         if kind == 'pcm':
             width = t.bit_depth // 8
             frames = len(table.data) // (t.channels * width)
