@@ -39,7 +39,7 @@
 extern "C" {
 #endif
 
-#define SB_ABI_VERSION 6
+#define SB_ABI_VERSION 7
 
 /* status codes */
 #define SB_OK            0
@@ -55,6 +55,7 @@ extern "C" {
 typedef struct sb_stream sb_stream;      /* opaque: one normalised stream in HBM */
 typedef struct sb_flac sb_flac;          /* opaque: an indexed FLAC file on the device */
 typedef struct sb_truehd sb_truehd;      /* opaque: a decoded TrueHD stream on the device */
+typedef struct sb_ts sb_ts;              /* opaque: one audio PID of an MPEG transport stream being demuxed */
 
 /* ---- life cycle ------------------------------------------------------- */
 
@@ -274,6 +275,37 @@ int sb_truehd_index(const void* buf, int64_t nbytes, const int64_t* offsets, con
                     int32_t* info, sb_truehd** out, int64_t* frames_out);
 int sb_truehd_decode(sb_truehd* thd, int sample_rate, int64_t padding, int64_t total_len, sb_stream** out_f32);
 int sb_truehd_destroy(sb_truehd* thd);
+
+/* ---- MPEG transport streams (ABI version 7) ----------------------------------
+ *
+ * One audio PID of a BDAV (192-byte packets: a 4-byte arrival time stamp, then the 188-byte packet) or plain
+ * (188-byte) transport stream, demuxed and decoded on the GPU.  The file is fed in chunks of whole packets, in order;
+ * the host does no per-packet work.  For each chunk k_ts_scan checks every packet's sync byte and, for the PID's
+ * packets, the transport error indicator, scrambling control, adaptation field length and continuity counter
+ * (carried across chunks; discontinuity_indicator honoured); the PID's payload bytes and packet table are appended on
+ * the device (the rest of the chunk is not kept).  sb_ts_finish parses every PES header (k_pes_index), checks
+ * PES_packet_length against the bytes the PID carried and then:
+ *   SB_TS_PCM_BLURAY  every PES's BD-LPCM header must give the first one's channel assignment, rate and bits; each
+ *                     PES gives its whole sample frames (leftover bytes are ignored) and k_bdlpcm_decode writes int16
+ *                     PCM (16-bit samples as they are, 24-bit samples their top 16 bits, the padding channel of an
+ *                     odd channel count dropped), as FFmpeg's pcm_bluray decoder returns them; 20-bit samples are
+ *                     refused, as FFmpeg's decoder refuses them;
+ *   SB_TS_TRUEHD      the payloads of the PES packets FFmpeg routes to the TrueHD stream (every stream_id_extension
+ *                     but 0x76, the AC-3 sub-stream) are one raw TrueHD stream, decoded as sb_truehd_index decodes a
+ *                     .thd file; AUs may straddle PES and TS packets.
+ * Damage fails with SB_EINVAL, sb_last_error() naming the byte offset of the packet (TS damage), of the PES's first
+ * packet (PES damage) or of the packet holding an AU's first byte (TrueHD damage).  A last PES shorter than its
+ * PES_packet_length (a cut file) keeps its whole sample frames and sets info[3]; one cut inside its header is dropped.
+ * sb_ts_feed returns once the chunk is copied, so the caller may refill its buffer while the GPU scans it.
+ * info[0..3] receive channels, sample rate, bits per coded sample and the cut flag; *frames_out the sample frames.
+ * sb_ts_decode resamples to sample_rate and pads exactly as sb_load_pcm does, into a SB_F32 stream. */
+#define SB_TS_PCM_BLURAY 0
+#define SB_TS_TRUEHD 1
+int sb_ts_open(int packet_size, int32_t pid, int32_t codec, sb_ts** out);
+int sb_ts_feed(sb_ts* ts, const void* host_chunk, int64_t nbytes, int64_t file_offset);
+int sb_ts_finish(sb_ts* ts, int32_t* info, int64_t* frames_out);
+int sb_ts_decode(sb_ts* ts, int sample_rate, int64_t padding, int64_t total_len, sb_stream** out_f32);
+int sb_ts_destroy(sb_ts* ts);
 
 /* ---- multi-GPU: events shard across ranks (SURVEY.md 8e) ---------------- */
 

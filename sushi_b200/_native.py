@@ -14,7 +14,8 @@ LIB_PATH = os.path.join(_HERE, 'libsushi_b200.so')
 
 SB_OK = 0
 SB_U8, SB_F32 = 0, 1
-ABI_VERSION = 6
+ABI_VERSION = 7
+SB_TS_PCM_BLURAY, SB_TS_TRUEHD = 0, 1
 
 c_i64 = ctypes.c_int64
 c_i64p = ctypes.POINTER(ctypes.c_int64)
@@ -74,6 +75,11 @@ PROTOTYPES = {
     'sb_truehd_index': (ctypes.c_int, [c_vp, c_i64, c_i64p, c_i64p, c_i64, c_i32p, ctypes.POINTER(c_vp), c_i64p]),
     'sb_truehd_decode': (ctypes.c_int, [c_vp, ctypes.c_int, c_i64, c_i64, ctypes.POINTER(c_vp)]),
     'sb_truehd_destroy': (ctypes.c_int, [c_vp]),
+    'sb_ts_open': (ctypes.c_int, [ctypes.c_int, ctypes.c_int32, ctypes.c_int32, ctypes.POINTER(c_vp)]),
+    'sb_ts_feed': (ctypes.c_int, [c_vp, c_vp, c_i64, c_i64]),
+    'sb_ts_finish': (ctypes.c_int, [c_vp, c_i32p, c_i64p]),
+    'sb_ts_decode': (ctypes.c_int, [c_vp, ctypes.c_int, c_i64, c_i64, ctypes.POINTER(c_vp)]),
+    'sb_ts_destroy': (ctypes.c_int, [c_vp]),
     'sb_comm_unique_id': (ctypes.c_int, [c_vp]),
     'sb_comm_init': (ctypes.c_int, [c_vp, ctypes.c_int, ctypes.c_int]),
     'sb_comm_destroy': (ctypes.c_int, []),

@@ -2,7 +2,7 @@
 
 Flags, defaults and checks are the reference's (sushi.py:528-843).  --src and --dst are WAV, FLAC or Matroska
 (.mkv, .mka, .mks, .webm) files.  For a WAV file the reference starts no subprocess either; a FLAC file or a
-Matroska file's FLAC or PCM track is decoded on the GPU, where the reference would have ffmpeg convert it to a WAV
+Matroska file's FLAC or PCM track, or a transport stream's (.m2ts, .mts, .m2t, .ts) BD-LPCM or TrueHD stream, is decoded on the GPU, where the reference would have ffmpeg convert it to a WAV
 file (DESIGN.md section 2): no WAV file is ever written.  A Matroska input also gives, as the reference's ffmpeg and
 mkvextract calls do, the script, the chapters and the video timestamps (sushi_b200.matroska); those are written to
 the reference's temporary paths and removed at the end unless --no-cleanup is given.  Every check runs before the GPU
@@ -16,7 +16,7 @@ import sys
 import time
 
 from . import __version__
-from . import matroska
+from . import matroska, mpegts
 from .common import SushiError
 from .pipeline import shift_script
 from .script import format_srt_time
@@ -108,9 +108,9 @@ def create_arg_parser():
                         help='Timecodes file to use instead of making one from the source (when possible)')
 
     parser.add_argument('--src', required=True, dest='source', metavar='<filename>',
-                        help='Source audio or video (WAV, FLAC, TrueHD or Matroska)')
+                        help='Source audio or video (WAV, FLAC, TrueHD, Matroska or MPEG-TS)')
     parser.add_argument('--dst', required=True, dest='destination', metavar='<filename>',
-                        help='Destination audio or video (WAV, FLAC, TrueHD or Matroska)')
+                        help='Destination audio or video (WAV, FLAC, TrueHD, Matroska or MPEG-TS)')
     parser.add_argument('-o', '--output', default=None, dest='output_script', metavar='<filename>',
                         help='Output script')
 
@@ -121,11 +121,18 @@ def create_arg_parser():
 
 
 def _open_input(path):
-    """None for a WAV, FLAC or raw TrueHD (.thd) input; the opened MatroskaFile for a Matroska one.  Anything else, or a Matroska name
-    that does not open as one, is refused where the reference would have ffmpeg demux it."""
+    """None for a WAV, FLAC or raw TrueHD (.thd) input; the opened MatroskaFile for a Matroska one, the opened
+    TransportStream for a transport stream (.m2ts, .mts, .m2t, .ts).  Anything else, or a Matroska or transport stream
+    name that does not open as one, is refused where the reference would have ffmpeg demux it."""
     ext = get_extension(path)
     if ext in ('.wav', '.flac', '.thd'):
         return None
+    if ext in mpegts.TS_EXTENSIONS:
+        try:
+            return mpegts.TransportStream(path)
+        except (OSError, SushiError) as e:
+            raise SushiError('{0}: demuxing is not supported, convert the input to WAV or FLAC first '
+                             '(it does not open as a transport stream: {1})'.format(path, e))
     if ext in MATROSKA_EXTENSIONS:
         try:
             return matroska.MatroskaFile(path)
@@ -136,11 +143,12 @@ def _open_input(path):
 
 
 def _select_audio(mkv, idx):
-    """The stream id of a Matroska input's audio track (None for WAV and FLAC), refusing what cannot be decoded."""
+    """The stream id of a Matroska or transport stream input's audio track (None for WAV and FLAC), refusing what
+    cannot be decoded."""
     if mkv is None:
         return None
     track = mkv.select('audio', idx)
-    matroska.audio_codec(track)
+    (mpegts if isinstance(mkv, mpegts.TransportStream) else matroska).audio_codec(track)
     return track.id
 
 
@@ -259,6 +267,9 @@ def _run(args, ignore_chapters, src_mkv, dst_mkv, written):
                 return external_file
             if fps_arg:
                 return None
+            if isinstance(mkv, mpegts.TransportStream):
+                raise SushiError('{0}: video timestamps cannot be read from a transport stream here; pass --src-fps / '
+                                 '--dst-fps or a timecodes file'.format(path))
             if mkv is not None and mkv.streams('video'):
                 out = format_full_path(args.temp_dir, path, '.sushi.timecodes.txt')
                 extract.append((out, mkv.timecodes_text))

@@ -1,6 +1,7 @@
 """Small helpers shared by the host side (mirror of the pieces of the reference's
 common.py that the hot path touches: SushiError common.py:4, clip common.py:41-42,
 format_time common.py:32-38 -- used only in log lines)."""
+import logging
 
 
 class SushiError(Exception):
@@ -23,3 +24,33 @@ def format_time(seconds):
     cs = py2_round(seconds * 100)
     return '{0}:{1:02d}:{2:02d}.{3:02d}'.format(
         int(cs // 360000), int((cs // 6000) % 60), int((cs // 100) % 60), int(cs % 100))
+
+
+def format_stream(t):
+    """One line of a stream candidate list: id, title, what the stream is."""
+    return '{0}{1}: {2}'.format(t.id, ' (%s)' % t.title if t.title else '', t.info)
+
+
+def select_stream(streams, kind, idx, path):
+    """The reference's Demuxer._select_stream (demux.py:335-355) over a container's streams of one kind (objects with
+    .id, .title, .info and .default): `idx` a stream id, or None for the only stream, else the default one."""
+    listing = '\n'.join(format_stream(t) for t in streams)
+    if not streams:
+        raise SushiError('No {0} streams found in {1}'.format(kind, path))
+    if idx is None:
+        if len(streams) > 1:
+            default = next((t for t in streams if t.default), None)
+            if default:
+                logging.warning('Using default track {0} in {1} because there are multiple candidates'
+                                .format(format_stream(default), path))
+                return default
+            raise SushiError('More than one {0} stream found in {1}.'
+                             'You need to specify the exact one to demux. Here are all candidates:\n'
+                             '{2}'.format(kind, path, listing))
+        return streams[0]
+    try:
+        return next(t for t in streams if t.id == idx)
+    except StopIteration:
+        raise SushiError("Stream with index {0} doesn't exist in {1}.\n"
+                         "Here are all that do:\n"
+                         "{2}".format(idx, path, listing))

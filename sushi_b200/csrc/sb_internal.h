@@ -6,6 +6,7 @@
 #include <string>
 #include <vector>
 #include <map>
+#include <functional>
 
 #include "sushi_b200.h"
 
@@ -137,6 +138,12 @@ void fused_release_tables();
 // sb_loader.cu: sb_load_pcm after its host-to-device copy (the FLAC decoder feeds it decoded int16 PCM on the device)
 int load_pcm_device(const unsigned char* d_pcm, int64_t frames, int channels, int sample_width, int framerate,
                     int sample_rate, int64_t padding, int64_t total_len, sb_stream** out_f32, const char* who);
+
+// sb_truehd.cu: sb_truehd_index on a stream already on the device (sb_ts.cu feeds it a transport stream's TrueHD
+// payload); where(off) names the file offset of stream byte `off` in messages
+int truehd_index_device(const uint8_t* host, const uint8_t* d_buf, int64_t nbytes, const int64_t* offsets,
+                        const int64_t* d_blocks, int64_t n, const std::function<int64_t(int64_t)>& where, int32_t* info,
+                        sb_truehd** out, int64_t* frames_out);
 
 }  // namespace sb
 

@@ -11,6 +11,7 @@
 #include "sb_internal.h"
 #include "sb_truehd.cuh"
 #include <algorithm>
+#include <functional>
 #include <new>
 #include <vector>
 
@@ -58,24 +59,15 @@ struct sb_truehd {
     int channels = 0, rate = 0;
 };
 
-extern "C" {
+namespace sb {
 
-int sb_truehd_index(const void* buf, int64_t nbytes, const int64_t* offsets, const int64_t* file_offsets, int64_t n,
-                    int32_t* info, sb_truehd** out, int64_t* frames_out) {
+// The body of sb_truehd_index on a stream already on the device: `host` and `d_buf` hold the same `nbytes` bytes (d_buf
+// zero-padded to 16 bytes past nbytes & ~3 for k_truehd_sync); blocks start at offsets[0..n) (d_blocks: the same on
+// the device); where(off) is the file offset messages give for stream byte `off`.  The caller keeps d_buf and d_blocks.
+int truehd_index_device(const uint8_t* host, const uint8_t* d_buf, int64_t nbytes, const int64_t* offsets,
+                        const int64_t* d_blocks, int64_t n, const std::function<int64_t(int64_t)>& where, int32_t* info,
+                        sb_truehd** out, int64_t* frames_out) {
     Ctx& c = ctx();
-    if (!c.inited) SB_FAIL(SB_ESTATE, "sb_truehd_index: library not initialised (call sb_init)");
-    if (!buf || !offsets || !file_offsets || !info || !out || !frames_out) SB_FAIL(SB_EINVAL, "sb_truehd_index: NULL argument");
-    if (nbytes < 1 || n < 1) SB_FAIL(SB_EINVAL, "sb_truehd_index: empty stream");
-    for (int64_t b = 0; b < n; ++b)
-        if (offsets[b] < 0 || offsets[b] >= nbytes || (b > 0 && offsets[b] <= offsets[b - 1]))
-            SB_FAIL(SB_EINVAL, "TrueHD block at byte offset %lld: %s", (long long)file_offsets[b],
-                    offsets[b] < 0 || offsets[b] >= nbytes ? "block starts outside the buffer" : "empty block");
-    const uint8_t* host = static_cast<const uint8_t*>(buf);
-    // the file offset of the block holding buffer offset `off`
-    auto where = [&](int64_t off) {
-        const int64_t b = std::upper_bound(offsets, offsets + n, off) - offsets;
-        return b > 0 && file_offsets[b - 1] >= 0 ? file_offsets[b - 1] : off;
-    };
     sbthd::Format f;
     char msg[256], fmsg[200];
     if (!sbthd::parse_format(host, nbytes, offsets[0], &f, fmsg, sizeof(fmsg))) {
@@ -85,15 +77,8 @@ int sb_truehd_index(const void* buf, int64_t nbytes, const int64_t* offsets, con
     sb_truehd* h = new (std::nothrow) sb_truehd();
     if (!h) SB_FAIL(SB_ENOMEM, "sb_truehd_index: out of host memory");
     h->channels = f.channels; h->rate = f.rate;
-    uint8_t* d_buf = nullptr;
-    int64_t* d_blocks = nullptr;
-    auto fail = [&](int code) { pool_free(d_buf); pool_free(d_blocks); sb_truehd_destroy(h); return code; };
-    if (pool_alloc((void**)&d_buf, (size_t)nbytes + 16) != SB_OK) return fail(SB_ENOMEM);
-    if (pool_alloc((void**)&d_blocks, sizeof(int64_t) * n + 16) != SB_OK) return fail(SB_ENOMEM);
-    cudaError_t e = cudaMemsetAsync(d_buf + (nbytes & ~(int64_t)3), 0, 16, c.stream);      // zero tail for k_truehd_sync
-    if (e == cudaSuccess) e = cudaMemcpyAsync(d_buf, buf, (size_t)nbytes, cudaMemcpyHostToDevice, c.stream);
-    if (e == cudaSuccess) e = cudaMemcpyAsync(d_blocks, offsets, sizeof(int64_t) * n, cudaMemcpyHostToDevice, c.stream);
-    if (e != cudaSuccess) { fail(0); SB_FAIL(SB_ECUDA, "sb_truehd_index: %s", cudaGetErrorString(e)); }
+    auto fail = [&](int code) { sb_truehd_destroy(h); return code; };
+    cudaError_t e = cudaSuccess;
 
     // candidates: a major sync opens every 1 to 128 AUs of at least a few dozen bytes
     int64_t cap = nbytes / 512 + 4096;
@@ -159,14 +144,48 @@ int sb_truehd_index(const void* buf, int64_t nbytes, const int64_t* offsets, con
         return where(off);
     };
     const int64_t frames = sbthd::check_segments(segs, status.data(), f, where_au, msg, sizeof(msg));
-    pool_free(d_buf); d_buf = nullptr;
-    pool_free(d_blocks); d_blocks = nullptr;
     if (frames < 0) { sb_truehd_destroy(h); SB_FAIL(SB_EINVAL, "%s", msg); }
     h->samples = frames;
     info[0] = f.channels; info[1] = f.rate;
     *frames_out = frames;
     *out = h;
     return SB_OK;
+}
+
+}  // namespace sb
+
+extern "C" {
+
+int sb_truehd_index(const void* buf, int64_t nbytes, const int64_t* offsets, const int64_t* file_offsets, int64_t n,
+                    int32_t* info, sb_truehd** out, int64_t* frames_out) {
+    Ctx& c = ctx();
+    if (!c.inited) SB_FAIL(SB_ESTATE, "sb_truehd_index: library not initialised (call sb_init)");
+    if (!buf || !offsets || !file_offsets || !info || !out || !frames_out) SB_FAIL(SB_EINVAL, "sb_truehd_index: NULL argument");
+    if (nbytes < 1 || n < 1) SB_FAIL(SB_EINVAL, "sb_truehd_index: empty stream");
+    for (int64_t b = 0; b < n; ++b)
+        if (offsets[b] < 0 || offsets[b] >= nbytes || (b > 0 && offsets[b] <= offsets[b - 1]))
+            SB_FAIL(SB_EINVAL, "TrueHD block at byte offset %lld: %s", (long long)file_offsets[b],
+                    offsets[b] < 0 || offsets[b] >= nbytes ? "block starts outside the buffer" : "empty block");
+    const uint8_t* host = static_cast<const uint8_t*>(buf);
+    // the file offset of the block holding buffer offset `off`
+    auto where = [&](int64_t off) {
+        const int64_t b = std::upper_bound(offsets, offsets + n, off) - offsets;
+        return b > 0 && file_offsets[b - 1] >= 0 ? file_offsets[b - 1] : off;
+    };
+    uint8_t* d_buf = nullptr;
+    int64_t* d_blocks = nullptr;
+    auto release = [&]() { pool_free(d_buf); pool_free(d_blocks); };
+    if (pool_alloc((void**)&d_buf, (size_t)nbytes + 16) != SB_OK || pool_alloc((void**)&d_blocks, sizeof(int64_t) * n + 16) != SB_OK) {
+        release();
+        SB_FAIL(SB_ENOMEM, "sb_truehd_index: out of device memory");
+    }
+    cudaError_t e = cudaMemsetAsync(d_buf + (nbytes & ~(int64_t)3), 0, 16, c.stream);      // zero tail for k_truehd_sync
+    if (e == cudaSuccess) e = cudaMemcpyAsync(d_buf, buf, (size_t)nbytes, cudaMemcpyHostToDevice, c.stream);
+    if (e == cudaSuccess) e = cudaMemcpyAsync(d_blocks, offsets, sizeof(int64_t) * n, cudaMemcpyHostToDevice, c.stream);
+    if (e != cudaSuccess) { release(); SB_FAIL(SB_ECUDA, "sb_truehd_index: %s", cudaGetErrorString(e)); }
+    const int rc = truehd_index_device(host, d_buf, nbytes, offsets, d_blocks, n, where, info, out, frames_out);
+    release();
+    return rc;
 }
 
 int sb_truehd_decode(sb_truehd* h, int sample_rate, int64_t padding, int64_t total_len, sb_stream** out_f32) {

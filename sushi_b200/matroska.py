@@ -24,7 +24,7 @@ import zlib
 
 import numpy as np
 
-from .common import SushiError, py2_round
+from .common import SushiError, py2_round, select_stream
 
 EBML_MAGIC = b'\x1a\x45\xdf\xa3'
 
@@ -642,33 +642,9 @@ class MatroskaFile(object):
     def streams(self, kind):
         return [t for t in self.tracks if t.kind == kind]
 
-    @staticmethod
-    def _format_stream(t):
-        return '{0}{1}: {2}'.format(t.id, ' (%s)' % t.title if t.title else '', t.info)
-
     def select(self, kind, idx):
         """The reference's Demuxer._select_stream (demux.py:335-355): kind is 'audio', 'subtitles' or 'video'."""
-        streams = self.streams(kind)
-        listing = '\n'.join(self._format_stream(t) for t in streams)
-        if not streams:
-            raise SushiError('No {0} streams found in {1}'.format(kind, self.path))
-        if idx is None:
-            if len(streams) > 1:
-                default = next((t for t in streams if t.default), None)
-                if default:
-                    logging.warning('Using default track {0} in {1} because there are multiple candidates'
-                                    .format(self._format_stream(default), self.path))
-                    return default
-                raise SushiError('More than one {0} stream found in {1}.'
-                                 'You need to specify the exact one to demux. Here are all candidates:\n'
-                                 '{2}'.format(kind, self.path, listing))
-            return streams[0]
-        try:
-            return next(t for t in streams if t.id == idx)
-        except StopIteration:
-            raise SushiError("Stream with index {0} doesn't exist in {1}.\n"
-                             "Here are all that do:\n"
-                             "{2}".format(idx, self.path, listing))
+        return select_stream(self.streams(kind), kind, idx, self.path)
 
     # -- side products ----------------------------------------------------------------------------------------------
     def script_text(self, track):

@@ -24,7 +24,7 @@ from time import time
 
 import numpy as np
 
-from . import _native, matroska, truehd
+from . import _native, matroska, mpegts, truehd
 from ._nvtx import nvtx_range
 from .common import SushiError, clip, py2_round
 
@@ -317,11 +317,17 @@ class WavStream(StreamGeometry):
         sb_normalise); loader='host' runs the NumPy mirror of the same arithmetic and uploads the
         result (kept as the cross-check; both give bit-identical .data).  A Matroska file loads its audio track
         `track` (a stream id; None: the only audio track, else the default one, as the reference selects); `path` may
-        also be an opened MatroskaFile, whose frames then come from one walk shared with the script and timecodes."""
+        also be an opened MatroskaFile, whose frames then come from one walk shared with the script and timecodes.  A
+        transport stream (.m2ts, .mts, .m2t, .ts, or an opened TransportStream) loads its audio stream `track` the
+        same way."""
         if sample_type not in _DTYPES:
             raise SushiError('Unknown sample type of WAV stream, must be uint8 or float32')
         self._handle = None
         before_read = time()
+        if isinstance(path, mpegts.TransportStream) or mpegts.is_transport_stream(path):
+            self._load_ts(path, sample_rate, sample_type, device, loader, track)
+            logging.info('Done reading transport stream {0} in {1}s'.format(path, time() - before_read))
+            return
         if isinstance(path, matroska.MatroskaFile) or matroska.is_matroska(path):
             self._load_matroska(path, sample_rate, sample_type, device, loader, track)
             logging.info('Done reading Matroska {0} in {1}s'.format(path, time() - before_read))
@@ -419,6 +425,46 @@ class WavStream(StreamGeometry):
             self._load_gpu_with(decode, n.value, int(info[1]), sample_rate, sample_type, device)
         finally:
             lib.sb_truehd_destroy(h)
+
+    def _load_ts(self, path, sample_rate, sample_type, device, loader, track):
+        """A transport stream's BD-LPCM or TrueHD stream loads exactly as the plain PCM WAV of the samples FFmpeg's
+        decoder returns.  The file is read in chunks of mpegts.CHUNK_BYTES into two page-locked buffers, one after the
+        other, so that the GPU scans one chunk while the next is read; demuxing and decoding are sb_ts_* on the GPU.
+        There is no host decoder, so loader='host' is refused."""
+        ts = path if isinstance(path, mpegts.TransportStream) else mpegts.TransportStream(path)
+        s = ts.select('audio', track)
+        kind = mpegts.audio_codec(s)
+        if loader != 'gpu':
+            raise SushiError("{0}: {1} input needs loader='gpu' (there is no host decoder)".format(
+                ts.path, 'TrueHD' if kind == 'truehd' else 'BD-LPCM'))
+        lib = _native.lib(device)
+        h = ctypes.c_void_p()
+        codec = _native.SB_TS_TRUEHD if kind == 'truehd' else _native.SB_TS_PCM_BLURAY
+        _native.check(lib.sb_ts_open(ts.packet_size, s.pid, codec, ctypes.byref(h)), 'sb_ts_open')
+        try:
+            size = max(ts.packet_size, mpegts.CHUNK_BYTES // ts.packet_size * ts.packet_size)
+            buffers = [_native.pinned_empty((size,), np.uint8) for _ in range(2)]
+            with nvtx_range('sushi_b200: sb_ts_feed'):
+                for view, pos in ts.chunks(buffers):
+                    arr = np.frombuffer(view, np.uint8)
+                    _native.check(lib.sb_ts_feed(h, arr.ctypes.data_as(ctypes.c_void_p), len(arr), pos), 'sb_ts_feed')
+            del buffers
+            info = np.zeros(4, np.int32)
+            n = ctypes.c_int64()
+            with nvtx_range('sushi_b200: sb_ts_finish'):
+                _native.check(lib.sb_ts_finish(h, info.ctypes.data_as(_native.c_i32p), ctypes.byref(n)), 'sb_ts_finish')
+            if info[3]:
+                logging.warning('{0}: the last PES packet of stream {1} is cut short; its whole sample frames are '
+                                'kept'.format(ts.path, s.id))
+
+            def decode(padding, total):
+                raw = ctypes.c_void_p()
+                with nvtx_range('sushi_b200: sb_ts_decode'):
+                    _native.check(lib.sb_ts_decode(h, sample_rate, padding, total, ctypes.byref(raw)), 'sb_ts_decode')
+                return raw
+            self._load_gpu_with(decode, n.value, int(info[1]), sample_rate, sample_type, device)
+        finally:
+            lib.sb_ts_destroy(h)
 
     def _load_matroska(self, path, sample_rate, sample_type, device, loader, track):
         """A Matroska audio track loads exactly as the plain PCM WAV of its decoded samples, frames concatenated in
