@@ -39,7 +39,7 @@
 extern "C" {
 #endif
 
-#define SB_ABI_VERSION 7
+#define SB_ABI_VERSION 8
 
 /* status codes */
 #define SB_OK            0
@@ -56,6 +56,7 @@ typedef struct sb_stream sb_stream;      /* opaque: one normalised stream in HBM
 typedef struct sb_flac sb_flac;          /* opaque: an indexed FLAC file on the device */
 typedef struct sb_truehd sb_truehd;      /* opaque: a decoded TrueHD stream on the device */
 typedef struct sb_ts sb_ts;              /* opaque: one audio PID of an MPEG transport stream being demuxed */
+typedef struct sb_alac sb_alac;          /* opaque: an indexed ALAC track on the device */
 
 /* ---- life cycle ------------------------------------------------------- */
 
@@ -306,6 +307,32 @@ int sb_ts_feed(sb_ts* ts, const void* host_chunk, int64_t nbytes, int64_t file_o
 int sb_ts_finish(sb_ts* ts, int32_t* info, int64_t* frames_out);
 int sb_ts_decode(sb_ts* ts, int sample_rate, int64_t padding, int64_t total_len, sb_stream** out_f32);
 int sb_ts_destroy(sb_ts* ts);
+
+/* ---- ALAC (Apple Lossless) and big-endian PCM (ABI version 8) ------------------
+ *
+ * An ALAC track loads exactly as the plain PCM WAV of the samples FFmpeg's `alac` decoder returns loads through
+ * sb_load_pcm: 16-bit samples as they are, 20-, 24- and 32-bit ones by the top 16 bits of FFmpeg's S32 sample,
+ * channels in FFmpeg's order.  `buf` holds the track's frames back to back (`nbytes` bytes): frame f starts at
+ * offsets[f] (increasing) and ends where frame f + 1 starts, the last at nbytes.  file_offsets[f] is the byte offset
+ * in the container file of the MP4 sample or Matroska block holding frame f: every error names it with the frame
+ * index.  config[0..6] is the ALACSpecificConfig: frameLength (1 to 65536), bitDepth (16, 20, 24, 32), pb, mb, kb,
+ * channels (1 to 8), sampleRate.
+ * sb_alac_index_frames uploads the frames and reads each one's sample count from its first element on the GPU;
+ * *frames_out receives the decoded samples per channel.  sb_alac_decode decodes every frame (one GPU thread each),
+ * then resamples to sample_rate and pads exactly as sb_load_pcm does, into a SB_F32 stream.  Either fails with
+ * SB_EINVAL on: an element tag other than SCE, CPE, LFE and END; more or fewer channels than the config declares; a
+ * sample count of 0 or above frameLength, or differing between elements; a prediction type other than 0 and 15; an
+ * invalid element header; a frame that reads past its bytes; a frame without END.  Bytes after END are ignored. */
+int sb_alac_index_frames(const void* buf, int64_t nbytes, const int64_t* offsets, const int64_t* file_offsets, int64_t n,
+                         const int32_t* config, sb_alac** out, int64_t* frames_out);
+int sb_alac_decode(sb_alac* alac, int sample_rate, int64_t padding, int64_t total_len, sb_stream** out_f32);
+int sb_alac_destroy(sb_alac* alac);
+
+/* sb_load_pcm for big-endian 16- or 24-bit interleaved PCM (QuickTime `twos` / `in24`, ISO `ipcm`): the result is
+ * bit for bit what sb_load_pcm gives on the byte-swapped data. */
+int sb_load_pcm_be(const void* pcm_host, int64_t frames, int channels, int sample_width,
+                   int framerate, int sample_rate, int64_t padding, int64_t total_len,
+                   sb_stream** out_f32);
 
 /* ---- multi-GPU: events shard across ranks (SURVEY.md 8e) ---------------- */
 

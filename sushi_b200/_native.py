@@ -14,7 +14,7 @@ LIB_PATH = os.path.join(_HERE, 'libsushi_b200.so')
 
 SB_OK = 0
 SB_U8, SB_F32 = 0, 1
-ABI_VERSION = 7
+ABI_VERSION = 8
 SB_TS_PCM_BLURAY, SB_TS_TRUEHD = 0, 1
 
 c_i64 = ctypes.c_int64
@@ -80,6 +80,11 @@ PROTOTYPES = {
     'sb_ts_finish': (ctypes.c_int, [c_vp, c_i32p, c_i64p]),
     'sb_ts_decode': (ctypes.c_int, [c_vp, ctypes.c_int, c_i64, c_i64, ctypes.POINTER(c_vp)]),
     'sb_ts_destroy': (ctypes.c_int, [c_vp]),
+    'sb_alac_index_frames': (ctypes.c_int, [c_vp, c_i64, c_i64p, c_i64p, c_i64, c_i32p, ctypes.POINTER(c_vp), c_i64p]),
+    'sb_alac_decode': (ctypes.c_int, [c_vp, ctypes.c_int, c_i64, c_i64, ctypes.POINTER(c_vp)]),
+    'sb_alac_destroy': (ctypes.c_int, [c_vp]),
+    'sb_load_pcm_be': (ctypes.c_int, [c_vp, c_i64, ctypes.c_int, ctypes.c_int, ctypes.c_int, ctypes.c_int,
+                                      c_i64, c_i64, ctypes.POINTER(c_vp)]),
     'sb_comm_unique_id': (ctypes.c_int, [c_vp]),
     'sb_comm_init': (ctypes.c_int, [c_vp, ctypes.c_int, ctypes.c_int]),
     'sb_comm_destroy': (ctypes.c_int, []),

@@ -1,9 +1,10 @@
 """The Sushi command line: `python -m sushi_b200 --src a.mkv --dst b.mkv -o out.ass`.
 
-Flags, defaults and checks are the reference's (sushi.py:528-843).  --src and --dst are WAV, FLAC or Matroska
-(.mkv, .mka, .mks, .webm) files.  For a WAV file the reference starts no subprocess either; a FLAC file or a
-Matroska file's FLAC or PCM track, or a transport stream's (.m2ts, .mts, .m2t, .ts) BD-LPCM or TrueHD stream, is decoded on the GPU, where the reference would have ffmpeg convert it to a WAV
-file (DESIGN.md section 2): no WAV file is ever written.  A Matroska input also gives, as the reference's ffmpeg and
+Flags, defaults and checks are the reference's (sushi.py:528-843).  --src and --dst are WAV, FLAC, Matroska
+(.mkv, .mka, .mks, .webm), MP4 / QuickTime (.mp4, .m4a, .m4v, .mov) or transport stream files.  For a WAV file the
+reference starts no subprocess either; a FLAC file, a Matroska file's FLAC, ALAC or PCM track, an MP4 file's ALAC, FLAC
+or PCM track, or a transport stream's (.m2ts, .mts, .m2t, .ts) BD-LPCM or TrueHD stream, is decoded on the GPU, where
+the reference would have ffmpeg convert it to a WAV file (DESIGN.md section 2): no WAV file is ever written.  A Matroska input also gives, as the reference's ffmpeg and
 mkvextract calls do, the script, the chapters and the video timestamps (sushi_b200.matroska); those are written to
 the reference's temporary paths and removed at the end unless --no-cleanup is given.  Every check runs before the GPU
 is touched; the run itself is pipeline.shift_script.
@@ -16,7 +17,7 @@ import sys
 import time
 
 from . import __version__
-from . import matroska, mpegts
+from . import matroska, mp4, mpegts
 from .common import SushiError
 from .pipeline import shift_script
 from .script import format_srt_time
@@ -108,9 +109,9 @@ def create_arg_parser():
                         help='Timecodes file to use instead of making one from the source (when possible)')
 
     parser.add_argument('--src', required=True, dest='source', metavar='<filename>',
-                        help='Source audio or video (WAV, FLAC, TrueHD, Matroska or MPEG-TS)')
+                        help='Source audio or video (WAV, FLAC, TrueHD, Matroska, MP4 or MPEG-TS)')
     parser.add_argument('--dst', required=True, dest='destination', metavar='<filename>',
-                        help='Destination audio or video (WAV, FLAC, TrueHD, Matroska or MPEG-TS)')
+                        help='Destination audio or video (WAV, FLAC, TrueHD, Matroska, MP4 or MPEG-TS)')
     parser.add_argument('-o', '--output', default=None, dest='output_script', metavar='<filename>',
                         help='Output script')
 
@@ -139,6 +140,12 @@ def _open_input(path):
         except (OSError, SushiError) as e:
             raise SushiError('{0}: demuxing is not supported, convert the input to WAV or FLAC first '
                              '(it does not open as a Matroska file: {1})'.format(path, e))
+    if ext in mp4.MP4_EXTENSIONS:
+        try:
+            return mp4.Mp4File(path)
+        except (OSError, SushiError) as e:
+            raise SushiError('{0}: demuxing is not supported, convert the input to WAV or FLAC first '
+                             '(it does not open as an MP4 file: {1})'.format(path, e))
     raise SushiError('{0}: demuxing is not supported, convert the input to WAV or FLAC first'.format(path))
 
 
@@ -148,7 +155,11 @@ def _select_audio(mkv, idx):
     if mkv is None:
         return None
     track = mkv.select('audio', idx)
-    (mpegts if isinstance(mkv, mpegts.TransportStream) else matroska).audio_codec(track)
+    if isinstance(mkv, mp4.Mp4File):
+        mp4.audio_codec(track)
+        mkv.check_edits(track)
+    else:
+        (mpegts if isinstance(mkv, mpegts.TransportStream) else matroska).audio_codec(track)
     return track.id
 
 
@@ -269,6 +280,9 @@ def _run(args, ignore_chapters, src_mkv, dst_mkv, written):
                 return None
             if isinstance(mkv, mpegts.TransportStream):
                 raise SushiError('{0}: video timestamps cannot be read from a transport stream here; pass --src-fps / '
+                                 '--dst-fps or a timecodes file'.format(path))
+            if isinstance(mkv, mp4.Mp4File):
+                raise SushiError('{0}: video timestamps cannot be read from an MP4 file here; pass --src-fps / '
                                  '--dst-fps or a timecodes file'.format(path))
             if mkv is not None and mkv.streams('video'):
                 out = format_full_path(args.temp_dir, path, '.sushi.timecodes.txt')

@@ -684,8 +684,8 @@ class MatroskaFile(object):
 
 
 def audio_codec(track):
-    """'flac', 'truehd' or 'pcm' for an audio track the GPU loader decodes (FLAC, Dolby TrueHD, little-endian integer
-    PCM of 16 or 24 bits);
+    """'flac', 'truehd', 'alac' or 'pcm' for an audio track the GPU loader decodes (FLAC, Dolby TrueHD, ALAC, whose
+    CodecPrivate is the ALACSpecificConfig, little-endian integer PCM of 16 or 24 bits);
     SushiError naming the track and its codec for anything else."""
     if track.refusal:
         raise SushiError(track.refusal)
@@ -693,11 +693,13 @@ def audio_codec(track):
         return 'flac'
     if track.codec_id == 'A_TRUEHD':
         return 'truehd'
+    if track.codec_id == 'A_ALAC' and len(track.codec_private) >= 24:
+        return 'alac'
     if track.codec_id == 'A_PCM/INT/LIT' and track.bit_depth in (16, 24) and track.channels >= 1:
         return 'pcm'
     what = track.codec_id + (' at {0} bits'.format(track.bit_depth) if track.codec_id.startswith('A_PCM') else '')
-    raise SushiError('Audio track {0} is {1}, which cannot be decoded here (FLAC, TrueHD and 16- or 24-bit '
-                     'little-endian PCM can): convert it to FLAC or WAV first'.format(track.id, what))
+    raise SushiError('Audio track {0} is {1}, which cannot be decoded here (FLAC, TrueHD, ALAC and 16- or '
+                     '24-bit little-endian PCM can): convert it to FLAC or WAV first'.format(track.id, what))
 
 
 def _ass_time(ns):

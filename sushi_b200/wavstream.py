@@ -24,7 +24,7 @@ from time import time
 
 import numpy as np
 
-from . import _native, matroska, mpegts, truehd
+from . import _native, matroska, mp4, mpegts, truehd
 from ._nvtx import nvtx_range
 from .common import SushiError, clip, py2_round
 
@@ -319,7 +319,7 @@ class WavStream(StreamGeometry):
         `track` (a stream id; None: the only audio track, else the default one, as the reference selects); `path` may
         also be an opened MatroskaFile, whose frames then come from one walk shared with the script and timecodes.  A
         transport stream (.m2ts, .mts, .m2t, .ts, or an opened TransportStream) loads its audio stream `track` the
-        same way."""
+        same way, and so does an MP4 / QuickTime file (.mp4, .m4a, .m4v, .mov, or an opened Mp4File)."""
         if sample_type not in _DTYPES:
             raise SushiError('Unknown sample type of WAV stream, must be uint8 or float32')
         self._handle = None
@@ -327,6 +327,10 @@ class WavStream(StreamGeometry):
         if isinstance(path, mpegts.TransportStream) or mpegts.is_transport_stream(path):
             self._load_ts(path, sample_rate, sample_type, device, loader, track)
             logging.info('Done reading transport stream {0} in {1}s'.format(path, time() - before_read))
+            return
+        if isinstance(path, mp4.Mp4File) or (not isinstance(path, matroska.MatroskaFile) and mp4.is_mp4(path)):
+            self._load_mp4(path, sample_rate, sample_type, device, loader, track)
+            logging.info('Done reading MP4 {0} in {1}s'.format(path, time() - before_read))
             return
         if isinstance(path, matroska.MatroskaFile) or matroska.is_matroska(path):
             self._load_matroska(path, sample_rate, sample_type, device, loader, track)
@@ -487,6 +491,8 @@ class WavStream(StreamGeometry):
                     raise SushiError("{0}: FLAC input needs loader='gpu' (there is no host FLAC decoder)".format(path))
             if kind == 'truehd' and loader != 'gpu':
                 raise SushiError("{0}: TrueHD input needs loader='gpu' (there is no host TrueHD decoder)".format(path))
+            if kind == 'alac' and loader != 'gpu':
+                raise SushiError("{0}: ALAC input needs loader='gpu' (there is no host ALAC decoder)".format(path))
             table = mkv.frames([t.id])[t.id]
             mkv.release([t.id])
         finally:
@@ -494,6 +500,10 @@ class WavStream(StreamGeometry):
                 mkv.close()
         if kind == 'flac':
             table.refuse_empty(path, 'FLAC')
+        if kind == 'alac':
+            table.refuse_empty(path, 'ALAC')
+            self._load_alac_frames(table, t.codec_private[:24], sample_rate, sample_type, device)
+            return
         if kind == 'truehd':
             table.refuse_empty(path, 'TrueHD')
             truehd.MajorSync(table.data[:64], '{0} track {1}'.format(path, t.id))
@@ -513,6 +523,10 @@ class WavStream(StreamGeometry):
                 self._load(mem, sample_rate, sample_type)
                 self._upload(device)
             return
+        self._load_flac_frames(table, info, sample_rate, sample_type, device)
+
+    def _load_flac_frames(self, table, info, sample_rate, sample_type, device):
+        """sb_flac_index_frames on a container's FLAC frames (table.block: each frame's file offset), then the loader."""
         lib = _native.lib(device)
         h = ctypes.c_void_p()
         n = ctypes.c_int64()
@@ -534,6 +548,97 @@ class WavStream(StreamGeometry):
             self._load_gpu_with(decode, n.value, info.framerate, sample_rate, sample_type, device)
         finally:
             lib.sb_flac_destroy(h)
+
+    def _load_alac_frames(self, table, cookie, sample_rate, sample_type, device):
+        """sb_alac_index_frames on a container's ALAC frames (cookie: the 24-byte ALACSpecificConfig; table.block:
+        each frame's file offset, which errors name), then the loader."""
+        fl, _, depth, pb, mb, kb, channels, _, _, _, rate = struct.unpack('>IBBBBBBHIII', cookie)
+        config = np.array([fl, depth, pb, mb, kb, channels, rate], np.int32)
+        lib = _native.lib(device)
+        h = ctypes.c_void_p()
+        n = ctypes.c_int64()
+        buf = np.frombuffer(table.data + b'\0', dtype=np.uint8)
+        offsets = np.ascontiguousarray(table.offset, np.int64)
+        blocks = np.ascontiguousarray(table.block, np.int64)
+        with nvtx_range('sushi_b200: sb_alac_index_frames'):
+            _native.check(lib.sb_alac_index_frames(buf.ctypes.data_as(ctypes.c_void_p), len(table.data) or 1,
+                                                   offsets.ctypes.data_as(_native.c_i64p),
+                                                   blocks.ctypes.data_as(_native.c_i64p), len(offsets),
+                                                   config.ctypes.data_as(_native.c_i32p), ctypes.byref(h),
+                                                   ctypes.byref(n)), 'sb_alac_index_frames')
+        try:
+            def decode(padding, total):
+                raw = ctypes.c_void_p()
+                with nvtx_range('sushi_b200: sb_alac_decode'):
+                    _native.check(lib.sb_alac_decode(h, sample_rate, padding, total, ctypes.byref(raw)), 'sb_alac_decode')
+                return raw
+            self._load_gpu_with(decode, n.value, rate, sample_rate, sample_type, device)
+        finally:
+            lib.sb_alac_destroy(h)
+
+    def _load_mp4(self, path, sample_rate, sample_type, device, loader, track):
+        """An MP4 / QuickTime audio track loads exactly as the plain PCM WAV of the samples FFmpeg's decoder returns.
+        ALAC and FLAC samples are decoded on the GPU where the sample table puts them; 16- and 24-bit PCM goes through
+        sb_load_pcm (little-endian) or sb_load_pcm_be (big-endian).  loader='host' works for PCM only.  `path` is a file
+        name or an opened Mp4File (left open)."""
+        opened = isinstance(path, mp4.Mp4File)
+        f = path if opened else mp4.Mp4File(path)
+        path = f.path
+        try:
+            t = f.select('audio', track)
+            kind = mp4.audio_codec(t)
+            f.check_edits(t)
+            if kind == 'flac':
+                info = FlacFile.from_bytes(t.config, '{0} track {1}'.format(path, t.id))
+                if info.bits_per_sample not in (16, 24):
+                    raise SushiError('FLAC with {0} bits per sample is not supported (16 or 24)'.format(
+                        info.bits_per_sample))
+            if kind != 'pcm' and loader != 'gpu':
+                raise SushiError("{0}: {1} input needs loader='gpu' (there is no host {1} decoder)".format(
+                    path, kind.upper()))
+            table = f.frames(t)
+        finally:
+            if not opened:
+                f.close()
+        if kind == 'alac':
+            table.refuse_empty(path, 'ALAC')
+            self._load_alac_frames(table, t.config, sample_rate, sample_type, device)
+            return
+        if kind == 'flac':
+            table.refuse_empty(path, 'FLAC')
+            self._load_flac_frames(table, info, sample_rate, sample_type, device)
+            return
+        width, big = mp4.PCM_DECODED[t.codec]
+        frames = len(table.data) // (t.channels * width)
+        data = table.data[:frames * t.channels * width]
+        if loader == 'gpu':
+            if big:
+                self._load_gpu_be(data, frames, t.channels, width, t.rate, sample_rate, sample_type, device)
+            else:
+                self._load_gpu(data, frames, t.channels, width, t.rate, sample_rate, sample_type, device)
+            return
+        if big:
+            data = np.frombuffer(data, np.uint8).reshape(-1, width)[:, ::-1].tobytes()
+        mem = DownmixedWavFile.__new__(DownmixedWavFile)
+        mem._file = io.BytesIO(data)
+        mem.channels_count, mem.framerate, mem.sample_width = t.channels, t.rate, width
+        mem.frame_size, mem.frames_count = t.channels * width, frames
+        self._load(mem, sample_rate, sample_type)
+        self._upload(device)
+
+    def _load_gpu_be(self, pcm, frames, channels, sample_width, framerate, sample_rate, sample_type, device):
+        """_load_gpu for big-endian PCM: sb_load_pcm_be."""
+        buf = np.frombuffer(pcm, dtype=np.uint8, count=frames * channels * sample_width)
+        lib = _native.lib(device)
+
+        def load(padding, total):
+            raw = ctypes.c_void_p()
+            with nvtx_range('sushi_b200: sb_load_pcm_be'):
+                _native.check(lib.sb_load_pcm_be(buf.ctypes.data_as(ctypes.c_void_p), frames, channels, sample_width,
+                                                 framerate, sample_rate, padding, total, ctypes.byref(raw)),
+                              'sb_load_pcm_be')
+            return raw
+        self._load_gpu_with(load, frames, framerate, sample_rate, sample_type, device)
 
     def _load_gpu(self, pcm, frames, channels, sample_width, framerate, sample_rate, sample_type, device):
         """wav.py:108-156 on the GPU: geometry here (same scalar code as the reference), arithmetic
