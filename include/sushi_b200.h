@@ -39,7 +39,7 @@
 extern "C" {
 #endif
 
-#define SB_ABI_VERSION 8
+#define SB_ABI_VERSION 9
 
 /* status codes */
 #define SB_OK            0
@@ -53,10 +53,8 @@ extern "C" {
 #define SB_F32 1             /* 'float32'                                    */
 
 typedef struct sb_stream sb_stream;      /* opaque: one normalised stream in HBM */
-typedef struct sb_flac sb_flac;          /* opaque: an indexed FLAC file on the device */
-typedef struct sb_truehd sb_truehd;      /* opaque: a decoded TrueHD stream on the device */
+typedef struct sb_pcm sb_pcm;            /* opaque: decoded interleaved int16 PCM on the device */
 typedef struct sb_ts sb_ts;              /* opaque: one audio PID of an MPEG transport stream being demuxed */
-typedef struct sb_alac sb_alac;          /* opaque: an indexed ALAC track on the device */
 
 /* ---- life cycle ------------------------------------------------------- */
 
@@ -228,54 +226,61 @@ int sb_load_pcm(const void* pcm_host, int64_t frames, int channels, int sample_w
 int sb_normalise(const sb_stream* raw_f32, int dtype, sb_stream** out,
                  float* min3_out, float* max3_out);
 
-/* ---- FLAC input (ABI version 3) -------------------------------------------
+/* ---- decoded input (ABI version 9) -------------------------------------------
  *
- * A FLAC file loads exactly as the plain PCM WAV of its decoded samples loads through sb_load_pcm: 16-bit samples
- * as they are, 24-bit ones by their top 16 bits.  Decoding runs on the GPU; the stream geometry stays with the
- * caller, as it does for WAV, so indexing (which yields the sample count) and decoding are two calls.
- *
- * sb_flac_index uploads the whole file (`nbytes` bytes, metadata included; the caller has read STREAMINFO and
- * passes its channel count, bits per sample and sample rate) and finds its frames: the first at
- * first_frame_offset, each next one by its coded frame or sample number.  *frames_out receives the decoded samples
- * per channel.  Only 16 and 24 bits per sample and 1 to 8 channels are accepted.
- * sb_flac_decode decodes every frame, checks each frame's CRC-16 and that it ends exactly where the next frame
- * (or the file) does, then resamples to sample_rate and pads exactly as sb_load_pcm does, into a SB_F32 stream for
- * sb_normalise.  A corrupt file fails with SB_EINVAL and sb_last_error() names the frame and its byte offset;
- * no samples are produced.  The STREAMINFO MD5 is not checked. */
-int sb_flac_index(const void* file, int64_t nbytes, int64_t first_frame_offset, int channels, int bits,
-                  int framerate, sb_flac** out, int64_t* frames_out);
-int sb_flac_decode(sb_flac* flac, int sample_rate, int64_t padding, int64_t total_len, sb_stream** out_f32);
-int sb_flac_destroy(sb_flac* flac);
+ * Every compressed input loads exactly as the plain PCM WAV of its decoded samples loads through sb_load_pcm.  A
+ * decoder is one call: it uploads the input, decodes it on the GPU, checks it completely and returns an sb_pcm
+ * handle, the decoded interleaved int16 PCM on the device (24-bit and wider samples keep their top 16 bits).  A
+ * damaged input fails with SB_EINVAL, sb_last_error() naming the frame or access unit and its byte offset, and no
+ * handle is returned.  The stream geometry stays with the caller, as it does for WAV: sb_pcm_info gives the sample
+ * frames, channels and rate it needs, and sb_pcm_load resamples to sample_rate and pads exactly as sb_load_pcm does,
+ * into a SB_F32 stream for sb_normalise.  The handle may be loaded any number of times until sb_pcm_destroy. */
+int sb_pcm_info(const sb_pcm* pcm, int64_t* frames, int32_t* channels, int32_t* rate);
+int sb_pcm_load(const sb_pcm* pcm, int sample_rate, int64_t padding, int64_t total_len, sb_stream** out_f32);
+int sb_pcm_destroy(sb_pcm* pcm);
 
-/* FLAC frames listed by a container (ABI version 5).  `buf` holds a track's frame payloads back to back (`nbytes`
- * bytes, no metadata); frame f starts at offsets[f] (increasing) and ends exactly where frame f + 1 starts, the last
- * at nbytes.  file_offsets[f] is the byte offset in the container file of the block holding frame f: every error
- * names it.  Each header must parse, agree with the stream parameters and pass its CRC-8 at its listed offset.  The
- * coded frame / sample numbers are not checked (a cut track starts above 0), and sample positions follow from the
- * block sizes.  The handle goes to sb_flac_decode and sb_flac_destroy as sb_flac_index's does; the decode then also
- * requires every frame to end exactly where its lace does. */
-int sb_flac_index_frames(const void* buf, int64_t nbytes, const int64_t* offsets, const int64_t* file_offsets, int64_t n,
-                         int channels, int bits, int framerate, sb_flac** out, int64_t* frames_out);
+/* Big-endian 16- or 24-bit interleaved PCM (QuickTime `twos` / `in24`, ISO `ipcm`): loaded through sb_pcm_load it
+ * gives bit for bit what sb_load_pcm gives on the byte-swapped data. */
+int sb_pcm_from_be(const void* pcm_host, int64_t frames, int channels, int sample_width, int framerate, sb_pcm** out);
 
-/* ---- Dolby TrueHD input (ABI version 6) ---------------------------------------
- *
- * A TrueHD stream loads exactly as the plain PCM WAV of the samples FFmpeg's decoder returns loads through
- * sb_load_pcm: the top 16 bits of each 24-bit sample, channels in FFmpeg's order, the presentation of substream
+/* FLAC (ABI version 3).  16 and 24 bits per sample and 1 to 8 channels are accepted; the caller has read STREAMINFO
+ * and passes its channel count, bits per sample and sample rate.  Every frame must decode, pass its CRC-16 and end
+ * exactly where the next frame (or the input) does.  The STREAMINFO MD5 is not checked.
+ * sb_flac_decode_file takes the whole file (`nbytes` bytes, metadata included) and finds its frames: the first at
+ * first_frame_offset, each next one by its coded frame or sample number.
+ * sb_flac_decode_frames (ABI version 5) takes frames a container lists.  `buf` holds a track's frame payloads back to
+ * back (`nbytes` bytes, no metadata); frame f starts at offsets[f] (increasing) and ends exactly where frame f + 1
+ * starts, the last at nbytes.  file_offsets[f] is the byte offset in the container file of the block holding frame
+ * f: every error names it.  Each header must parse, agree with the stream parameters and pass its CRC-8 at its listed
+ * offset.  The coded frame / sample numbers are not checked (a cut track starts above 0), and sample positions follow
+ * from the block sizes. */
+int sb_flac_decode_file(const void* file, int64_t nbytes, int64_t first_frame_offset, int channels, int bits,
+                        int framerate, sb_pcm** out);
+int sb_flac_decode_frames(const void* buf, int64_t nbytes, const int64_t* offsets, const int64_t* file_offsets, int64_t n,
+                          int channels, int bits, int framerate, sb_pcm** out);
+
+/* Dolby TrueHD (ABI version 6): FFmpeg's decoder output, channels in FFmpeg's order, the presentation of substream
  * min(n - 1, 2) (a fourth, object substream is skipped).  `buf` holds the stream's bytes (`nbytes`); a container's
- * blocks start at offsets[0..n) (increasing, back to back; a raw .thd stream is one block at 0) and
- * file_offsets[b] is the byte offset in the file of block b, which errors name (a negative one: errors name the
- * AU's own offset, as for a raw stream).  An access unit (AU) must end inside its block.
- * sb_truehd_index uploads the stream, lists its major syncs on the GPU, chains the AUs into restart segments on the
- * host and decodes every segment on the GPU, one thread each.  It fails with SB_EINVAL, sb_last_error() naming the
- * AU index and byte offset, on any damage listed in DESIGN.md section 2: check nibble, major sync CRC, restart header
- * checksum, substream parity or CRC, lossless check, AU lengths, a segment without restart headers, a short AU
- * before the end.  MLP is refused.  info[0..1] receive the channel count and the sample rate; *frames_out the
- * decoded samples per channel.
- * sb_truehd_decode resamples to sample_rate and pads exactly as sb_load_pcm does, into a SB_F32 stream. */
-int sb_truehd_index(const void* buf, int64_t nbytes, const int64_t* offsets, const int64_t* file_offsets, int64_t n,
-                    int32_t* info, sb_truehd** out, int64_t* frames_out);
-int sb_truehd_decode(sb_truehd* thd, int sample_rate, int64_t padding, int64_t total_len, sb_stream** out_f32);
-int sb_truehd_destroy(sb_truehd* thd);
+ * blocks start at offsets[0..n) (increasing, back to back; a raw .thd stream is one block at 0) and file_offsets[b]
+ * is the byte offset in the file of block b, which errors name (a negative one: errors name the AU's own offset, as
+ * for a raw stream).  An access unit (AU) must end inside its block.  The call lists the major syncs on the GPU,
+ * chains the AUs into restart segments on the host and decodes every segment on the GPU, one thread each.  It fails on
+ * any damage listed in DESIGN.md section 2: check nibble, major sync CRC, restart header checksum, substream parity or
+ * CRC, lossless check, AU lengths, a segment without restart headers, a short AU before the end.  MLP is refused. */
+int sb_truehd_decode(const void* buf, int64_t nbytes, const int64_t* offsets, const int64_t* file_offsets, int64_t n,
+                     sb_pcm** out);
+
+/* ALAC, Apple Lossless (ABI version 8): FFmpeg's `alac` decoder output, 20-, 24- and 32-bit samples by the top 16
+ * bits of FFmpeg's S32 sample, channels in FFmpeg's order.  `buf` holds the track's frames back to back (`nbytes`
+ * bytes): frame f starts at offsets[f] (increasing) and ends where frame f + 1 starts, the last at nbytes.
+ * file_offsets[f] is the byte offset in the container file of the MP4 sample or Matroska block holding frame f: every
+ * error names it with the frame index.  config[0..6] is the ALACSpecificConfig: frameLength (1 to 65536), bitDepth
+ * (16, 20, 24, 32), pb, mb, kb, channels (1 to 8), sampleRate.  One GPU thread decodes each frame.  It fails on: an
+ * element tag other than SCE, CPE, LFE and END; more or fewer channels than the config declares; a sample count of 0
+ * or above frameLength, or differing between elements; a prediction type other than 0 and 15; an invalid element
+ * header; a frame that reads past its bytes; a frame without END.  Bytes after END are ignored. */
+int sb_alac_decode_frames(const void* buf, int64_t nbytes, const int64_t* offsets, const int64_t* file_offsets, int64_t n,
+                          const int32_t* config, sb_pcm** out);
 
 /* ---- MPEG transport streams (ABI version 7) ----------------------------------
  *
@@ -285,54 +290,26 @@ int sb_truehd_destroy(sb_truehd* thd);
  * packets, the transport error indicator, scrambling control, adaptation field length and continuity counter
  * (carried across chunks; discontinuity_indicator honoured); the PID's payload bytes and packet table are appended on
  * the device (the rest of the chunk is not kept).  sb_ts_finish parses every PES header (k_pes_index), checks
- * PES_packet_length against the bytes the PID carried and then:
+ * PES_packet_length against the bytes the PID carried and returns the decoded PCM as an sb_pcm:
  *   SB_TS_PCM_BLURAY  every PES's BD-LPCM header must give the first one's channel assignment, rate and bits; each
  *                     PES gives its whole sample frames (leftover bytes are ignored) and k_bdlpcm_decode writes int16
  *                     PCM (16-bit samples as they are, 24-bit samples their top 16 bits, the padding channel of an
  *                     odd channel count dropped), as FFmpeg's pcm_bluray decoder returns them; 20-bit samples are
  *                     refused, as FFmpeg's decoder refuses them;
  *   SB_TS_TRUEHD      the payloads of the PES packets FFmpeg routes to the TrueHD stream (every stream_id_extension
- *                     but 0x76, the AC-3 sub-stream) are one raw TrueHD stream, decoded as sb_truehd_index decodes a
+ *                     but 0x76, the AC-3 sub-stream) are one raw TrueHD stream, decoded as sb_truehd_decode decodes a
  *                     .thd file; AUs may straddle PES and TS packets.
  * Damage fails with SB_EINVAL, sb_last_error() naming the byte offset of the packet (TS damage), of the PES's first
  * packet (PES damage) or of the packet holding an AU's first byte (TrueHD damage).  A last PES shorter than its
- * PES_packet_length (a cut file) keeps its whole sample frames and sets info[3]; one cut inside its header is dropped.
- * sb_ts_feed returns once the chunk is copied, so the caller may refill its buffer while the GPU scans it.
- * info[0..3] receive channels, sample rate, bits per coded sample and the cut flag; *frames_out the sample frames.
- * sb_ts_decode resamples to sample_rate and pads exactly as sb_load_pcm does, into a SB_F32 stream. */
+ * PES_packet_length (a cut file) keeps its whole sample frames and sets *cut; one cut inside its header is dropped.
+ * sb_ts_feed returns once the chunk is copied, so the caller may refill its buffer while the GPU scans it.  The sb_pcm
+ * outlives the sb_ts. */
 #define SB_TS_PCM_BLURAY 0
 #define SB_TS_TRUEHD 1
 int sb_ts_open(int packet_size, int32_t pid, int32_t codec, sb_ts** out);
 int sb_ts_feed(sb_ts* ts, const void* host_chunk, int64_t nbytes, int64_t file_offset);
-int sb_ts_finish(sb_ts* ts, int32_t* info, int64_t* frames_out);
-int sb_ts_decode(sb_ts* ts, int sample_rate, int64_t padding, int64_t total_len, sb_stream** out_f32);
+int sb_ts_finish(sb_ts* ts, int32_t* cut, sb_pcm** out);
 int sb_ts_destroy(sb_ts* ts);
-
-/* ---- ALAC (Apple Lossless) and big-endian PCM (ABI version 8) ------------------
- *
- * An ALAC track loads exactly as the plain PCM WAV of the samples FFmpeg's `alac` decoder returns loads through
- * sb_load_pcm: 16-bit samples as they are, 20-, 24- and 32-bit ones by the top 16 bits of FFmpeg's S32 sample,
- * channels in FFmpeg's order.  `buf` holds the track's frames back to back (`nbytes` bytes): frame f starts at
- * offsets[f] (increasing) and ends where frame f + 1 starts, the last at nbytes.  file_offsets[f] is the byte offset
- * in the container file of the MP4 sample or Matroska block holding frame f: every error names it with the frame
- * index.  config[0..6] is the ALACSpecificConfig: frameLength (1 to 65536), bitDepth (16, 20, 24, 32), pb, mb, kb,
- * channels (1 to 8), sampleRate.
- * sb_alac_index_frames uploads the frames and reads each one's sample count from its first element on the GPU;
- * *frames_out receives the decoded samples per channel.  sb_alac_decode decodes every frame (one GPU thread each),
- * then resamples to sample_rate and pads exactly as sb_load_pcm does, into a SB_F32 stream.  Either fails with
- * SB_EINVAL on: an element tag other than SCE, CPE, LFE and END; more or fewer channels than the config declares; a
- * sample count of 0 or above frameLength, or differing between elements; a prediction type other than 0 and 15; an
- * invalid element header; a frame that reads past its bytes; a frame without END.  Bytes after END are ignored. */
-int sb_alac_index_frames(const void* buf, int64_t nbytes, const int64_t* offsets, const int64_t* file_offsets, int64_t n,
-                         const int32_t* config, sb_alac** out, int64_t* frames_out);
-int sb_alac_decode(sb_alac* alac, int sample_rate, int64_t padding, int64_t total_len, sb_stream** out_f32);
-int sb_alac_destroy(sb_alac* alac);
-
-/* sb_load_pcm for big-endian 16- or 24-bit interleaved PCM (QuickTime `twos` / `in24`, ISO `ipcm`): the result is
- * bit for bit what sb_load_pcm gives on the byte-swapped data. */
-int sb_load_pcm_be(const void* pcm_host, int64_t frames, int channels, int sample_width,
-                   int framerate, int sample_rate, int64_t padding, int64_t total_len,
-                   sb_stream** out_f32);
 
 /* ---- multi-GPU: events shard across ranks (SURVEY.md 8e) ---------------- */
 

@@ -14,7 +14,7 @@ LIB_PATH = os.path.join(_HERE, 'libsushi_b200.so')
 
 SB_OK = 0
 SB_U8, SB_F32 = 0, 1
-ABI_VERSION = 8
+ABI_VERSION = 9
 SB_TS_PCM_BLURAY, SB_TS_TRUEHD = 0, 1
 
 c_i64 = ctypes.c_int64
@@ -66,25 +66,20 @@ PROTOTYPES = {
     'sb_load_pcm': (ctypes.c_int, [c_vp, c_i64, ctypes.c_int, ctypes.c_int, ctypes.c_int, ctypes.c_int,
                                    c_i64, c_i64, ctypes.POINTER(c_vp)]),
     'sb_normalise': (ctypes.c_int, [c_vp, ctypes.c_int, ctypes.POINTER(c_vp), c_f32p, c_f32p]),
-    'sb_flac_index': (ctypes.c_int, [c_vp, c_i64, c_i64, ctypes.c_int, ctypes.c_int, ctypes.c_int, ctypes.POINTER(c_vp),
-                                     c_i64p]),
-    'sb_flac_index_frames': (ctypes.c_int, [c_vp, c_i64, c_i64p, c_i64p, c_i64, ctypes.c_int, ctypes.c_int, ctypes.c_int,
-                                            ctypes.POINTER(c_vp), c_i64p]),
-    'sb_flac_decode': (ctypes.c_int, [c_vp, ctypes.c_int, c_i64, c_i64, ctypes.POINTER(c_vp)]),
-    'sb_flac_destroy': (ctypes.c_int, [c_vp]),
-    'sb_truehd_index': (ctypes.c_int, [c_vp, c_i64, c_i64p, c_i64p, c_i64, c_i32p, ctypes.POINTER(c_vp), c_i64p]),
-    'sb_truehd_decode': (ctypes.c_int, [c_vp, ctypes.c_int, c_i64, c_i64, ctypes.POINTER(c_vp)]),
-    'sb_truehd_destroy': (ctypes.c_int, [c_vp]),
+    'sb_pcm_info': (ctypes.c_int, [c_vp, c_i64p, c_i32p, c_i32p]),
+    'sb_pcm_load': (ctypes.c_int, [c_vp, ctypes.c_int, c_i64, c_i64, ctypes.POINTER(c_vp)]),
+    'sb_pcm_destroy': (ctypes.c_int, [c_vp]),
+    'sb_pcm_from_be': (ctypes.c_int, [c_vp, c_i64, ctypes.c_int, ctypes.c_int, ctypes.c_int, ctypes.POINTER(c_vp)]),
+    'sb_flac_decode_file': (ctypes.c_int, [c_vp, c_i64, c_i64, ctypes.c_int, ctypes.c_int, ctypes.c_int,
+                                           ctypes.POINTER(c_vp)]),
+    'sb_flac_decode_frames': (ctypes.c_int, [c_vp, c_i64, c_i64p, c_i64p, c_i64, ctypes.c_int, ctypes.c_int, ctypes.c_int,
+                                             ctypes.POINTER(c_vp)]),
+    'sb_truehd_decode': (ctypes.c_int, [c_vp, c_i64, c_i64p, c_i64p, c_i64, ctypes.POINTER(c_vp)]),
+    'sb_alac_decode_frames': (ctypes.c_int, [c_vp, c_i64, c_i64p, c_i64p, c_i64, c_i32p, ctypes.POINTER(c_vp)]),
     'sb_ts_open': (ctypes.c_int, [ctypes.c_int, ctypes.c_int32, ctypes.c_int32, ctypes.POINTER(c_vp)]),
     'sb_ts_feed': (ctypes.c_int, [c_vp, c_vp, c_i64, c_i64]),
-    'sb_ts_finish': (ctypes.c_int, [c_vp, c_i32p, c_i64p]),
-    'sb_ts_decode': (ctypes.c_int, [c_vp, ctypes.c_int, c_i64, c_i64, ctypes.POINTER(c_vp)]),
+    'sb_ts_finish': (ctypes.c_int, [c_vp, c_i32p, ctypes.POINTER(c_vp)]),
     'sb_ts_destroy': (ctypes.c_int, [c_vp]),
-    'sb_alac_index_frames': (ctypes.c_int, [c_vp, c_i64, c_i64p, c_i64p, c_i64, c_i32p, ctypes.POINTER(c_vp), c_i64p]),
-    'sb_alac_decode': (ctypes.c_int, [c_vp, ctypes.c_int, c_i64, c_i64, ctypes.POINTER(c_vp)]),
-    'sb_alac_destroy': (ctypes.c_int, [c_vp]),
-    'sb_load_pcm_be': (ctypes.c_int, [c_vp, c_i64, ctypes.c_int, ctypes.c_int, ctypes.c_int, ctypes.c_int,
-                                      c_i64, c_i64, ctypes.POINTER(c_vp)]),
     'sb_comm_unique_id': (ctypes.c_int, [c_vp]),
     'sb_comm_init': (ctypes.c_int, [c_vp, ctypes.c_int, ctypes.c_int]),
     'sb_comm_destroy': (ctypes.c_int, []),

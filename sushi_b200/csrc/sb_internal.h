@@ -11,6 +11,7 @@
 #include "sushi_b200.h"
 
 struct sb_stream;
+struct sb_pcm;
 
 namespace sb {
 
@@ -135,17 +136,26 @@ int launch_part_spectra(const sb_stream* tmpl, const QueryDesc* d_desc, int q_be
                         int64_t part_first, int64_t rows, float2* out);
 void fused_release_tables();
 
-// sb_loader.cu: sb_load_pcm after its host-to-device copy (the FLAC decoder feeds it decoded int16 PCM on the device)
+// sb_loader.cu: sb_load_pcm after its host-to-device copy (sb_pcm_load feeds it a decoder's int16 PCM on the device)
 int load_pcm_device(const unsigned char* d_pcm, int64_t frames, int channels, int sample_width, int framerate,
                     int sample_rate, int64_t padding, int64_t total_len, sb_stream** out_f32, const char* who);
 
-// sb_truehd.cu: sb_truehd_index on a stream already on the device (sb_ts.cu feeds it a transport stream's TrueHD
+// sb_loader.cu: a decoded-PCM handle that takes ownership of d_pcm (a pool block); on failure d_pcm is freed
+int pcm_handle(int16_t* d_pcm, int64_t frames, int channels, int rate, sb_pcm** out);
+
+// sb_truehd.cu: sb_truehd_decode on a stream already on the device (sb_ts.cu feeds it a transport stream's TrueHD
 // payload); where(off) names the file offset of stream byte `off` in messages
 int truehd_index_device(const uint8_t* host, const uint8_t* d_buf, int64_t nbytes, const int64_t* offsets,
-                        const int64_t* d_blocks, int64_t n, const std::function<int64_t(int64_t)>& where, int32_t* info,
-                        sb_truehd** out, int64_t* frames_out);
+                        const int64_t* d_blocks, int64_t n, const std::function<int64_t(int64_t)>& where, sb_pcm** out);
 
 }  // namespace sb
+
+// The decoded-PCM handle of the ABI: interleaved int16 PCM on the device, what every decoder produces.
+struct sb_pcm {
+    int16_t* d_pcm;
+    int64_t frames;
+    int channels, rate;
+};
 
 // The opaque stream handle of the ABI.
 struct sb_stream {

@@ -2,9 +2,11 @@
 //   K1  sb_load_pcm   int16/int24 decode, channel average, per-chunk nearest-neighbour resample
 //                     (cv2.resize INTER_NEAREST index map), edge padding      wav.py:64-91,125-141
 //   K2  sb_normalise  3 x median clip, rescale to [0,1], optional uint8 quantisation  wav.py:145-156
+// sb_pcm_load runs K1 on a decoder's int16 PCM (an sb_pcm); sb_pcm_from_be makes one from big-endian PCM (k_pcm_be).
 // Everything is float32 with explicitly rounded operations (no FMA contraction), in the order the
 // reference applies them, so the result is bit-identical to the NumPy/OpenCV loader.
 #include "sb_internal.h"
+#include <algorithm>
 #include <cmath>
 #include <cstring>
 #include <vector>
@@ -329,6 +331,15 @@ int plan_load(int64_t frames, int channels, int sample_width, int framerate, int
     return SB_OK;
 }
 
+// big-endian 16- or 24-bit samples -> the top 16 bits as int16
+__global__ void __launch_bounds__(256)
+k_pcm_be(const uint8_t* __restrict__ in, int64_t n, int width, int16_t* __restrict__ out) {
+    for (int64_t i = (int64_t)blockIdx.x * blockDim.x + threadIdx.x; i < n; i += (int64_t)gridDim.x * blockDim.x) {
+        const uint8_t* p = in + i * width;
+        out[i] = (int16_t)(uint16_t)(((unsigned)p[0] << 8) | p[1]);
+    }
+}
+
 }  // namespace
 
 namespace sb {
@@ -358,6 +369,13 @@ int load_pcm_device(const unsigned char* d_pcm, int64_t frames, int channels, in
     return SB_OK;
 }
 
+int pcm_handle(int16_t* d_pcm, int64_t frames, int channels, int rate, sb_pcm** out) {
+    sb_pcm* p = new (std::nothrow) sb_pcm{d_pcm, frames, channels, rate};
+    if (!p) { pool_free(d_pcm); SB_FAIL(SB_ENOMEM, "out of host memory for a decoded-PCM handle"); }
+    *out = p;
+    return SB_OK;
+}
+
 }  // namespace sb
 
 extern "C" {
@@ -384,6 +402,57 @@ int sb_load_pcm(const void* pcm_host, int64_t frames, int channels, int sample_w
     if (e != cudaSuccess) { sb_stream_destroy(s); SB_FAIL(SB_ECUDA, "sb_load_pcm: %s", cudaGetErrorString(e)); }
     *out_f32 = s;
     return SB_OK;
+}
+
+int sb_pcm_info(const sb_pcm* pcm, int64_t* frames, int32_t* channels, int32_t* rate) {
+    if (!pcm || !frames || !channels || !rate) SB_FAIL(SB_EINVAL, "sb_pcm_info: NULL argument");
+    *frames = pcm->frames; *channels = pcm->channels; *rate = pcm->rate;
+    return SB_OK;
+}
+
+int sb_pcm_load(const sb_pcm* pcm, int sample_rate, int64_t padding, int64_t total_len, sb_stream** out_f32) {
+    Ctx& c = ctx();
+    if (!c.inited) SB_FAIL(SB_ESTATE, "sb_pcm_load: library not initialised (call sb_init)");
+    if (!pcm || !out_f32) SB_FAIL(SB_EINVAL, "sb_pcm_load: NULL argument");
+    sb_stream* s = nullptr;
+    SB_TRY(load_pcm_device(reinterpret_cast<const unsigned char*>(pcm->d_pcm), pcm->frames, pcm->channels, 2, pcm->rate,
+                           sample_rate, padding, total_len, &s, "sb_pcm_load"));
+    const cudaError_t e = cudaStreamSynchronize(c.stream);
+    if (e != cudaSuccess) { sb_stream_destroy(s); SB_FAIL(SB_ECUDA, "sb_pcm_load: %s", cudaGetErrorString(e)); }
+    *out_f32 = s;
+    return SB_OK;
+}
+
+int sb_pcm_destroy(sb_pcm* pcm) {
+    if (!pcm) return SB_OK;
+    pool_free(pcm->d_pcm);
+    delete pcm;
+    return SB_OK;
+}
+
+int sb_pcm_from_be(const void* pcm_host, int64_t frames, int channels, int sample_width, int framerate, sb_pcm** out) {
+    Ctx& c = ctx();
+    if (!c.inited) SB_FAIL(SB_ESTATE, "sb_pcm_from_be: library not initialised (call sb_init)");
+    if (!pcm_host || !out) SB_FAIL(SB_EINVAL, "sb_pcm_from_be: NULL argument");
+    if (sample_width != 2 && sample_width != 3) SB_FAIL(SB_EINVAL, "Unsupported sample width: %d", sample_width);
+    if (frames < 0 || channels < 1) SB_FAIL(SB_EINVAL, "sb_pcm_from_be: bad geometry");
+    const int64_t n = frames * channels;
+    unsigned char* d_in = nullptr;
+    int16_t* d_pcm = nullptr;
+    int rc = pool_alloc((void**)&d_in, (size_t)n * sample_width + 16);
+    if (rc == SB_OK) rc = pool_alloc((void**)&d_pcm, sizeof(int16_t) * (size_t)n + 16);
+    if (rc != SB_OK) { pool_free(d_in); pool_free(d_pcm); return rc; }
+    cudaError_t e = cudaMemcpyAsync(d_in, pcm_host, (size_t)n * sample_width, cudaMemcpyHostToDevice, c.stream);
+    if (e == cudaSuccess && n > 0) {
+        ProfScope ps("pcm_be");
+        const int grid = (int)std::max<int64_t>(1, std::min<int64_t>((n + 255) / 256, (int64_t)c.sm_count * 16));
+        k_pcm_be<<<grid, 256, 0, c.stream>>>(d_in, n, sample_width, d_pcm);
+        e = cudaGetLastError();
+    }
+    if (e == cudaSuccess) e = cudaStreamSynchronize(c.stream);             // pcm_host may be reused by the caller
+    pool_free(d_in);
+    if (e != cudaSuccess) { pool_free(d_pcm); SB_FAIL(SB_ECUDA, "sb_pcm_from_be: %s", cudaGetErrorString(e)); }
+    return pcm_handle(d_pcm, frames, channels, framerate, out);
 }
 
 int sb_normalise(const sb_stream* raw_f32, int dtype, sb_stream** out, float* min3_out, float* max3_out) {

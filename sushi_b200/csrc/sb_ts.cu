@@ -12,8 +12,8 @@
 //                  and returns once the chunk is copied; the running totals come back before the next chunk is placed
 //   sb_ts_finish   k_pes_index (one thread per PES: header, PES_packet_length, BD-LPCM header or TrueHD routing), an
 //                  exclusive scan of each PES's sample frames (or kept bytes), then k_bdlpcm_decode (a grid-stride loop
-//                  over sample frames into interleaved int16) or k_ts_gather + the TrueHD decoder of sb_truehd.cu
-//   sb_ts_decode   the loader's own kernel (k_decode_resample_pad, width 2) on the int16 PCM
+//                  over sample frames into interleaved int16) or k_ts_gather + the TrueHD decoder of sb_truehd.cu, into
+//                  an sb_pcm
 // The per-packet and per-PES rules are in sb_ts.cuh, shared with the CPU emulation of the tests.
 #include "sb_internal.h"
 #include "sb_ts.cuh"
@@ -278,11 +278,6 @@ struct sb_ts {
     Totals* h_run = nullptr;                            // pinned copy of d_run[1]
     cudaEvent_t done = nullptr, copied = nullptr;
     bool pending = false, finished = false;
-    // after sb_ts_finish
-    int16_t* d_pcm = nullptr;
-    int64_t frames = 0;
-    int channels = 0, rate = 0;
-    sb_truehd* thd = nullptr;
 
     void release_demux() {
         pool_free(d_chunk); pool_free(d_info); pool_free(d_cta); pool_free(d_es); pool_free(d_tab); pool_free(d_pes);
@@ -406,10 +401,10 @@ int scan_i64(int64_t* d_v, int64_t n, int64_t* total) {
 
 extern "C" {
 
-int sb_ts_finish(sb_ts* t, int32_t* info, int64_t* frames_out) {
+int sb_ts_finish(sb_ts* t, int32_t* cut, sb_pcm** out) {
     Ctx& c = ctx();
     if (!c.inited) SB_FAIL(SB_ESTATE, "sb_ts_finish: library not initialised (call sb_init)");
-    if (!t || !info || !frames_out) SB_FAIL(SB_EINVAL, "sb_ts_finish: NULL argument");
+    if (!t || !cut || !out) SB_FAIL(SB_EINVAL, "sb_ts_finish: NULL argument");
     if (t->finished) SB_FAIL(SB_ESTATE, "sb_ts_finish: the stream is finished");
     t->finished = true;
     unsigned long long err = kNoError;
@@ -453,11 +448,12 @@ int sb_ts_finish(sb_ts* t, int32_t* info, int64_t* frames_out) {
     int64_t total = 0;
     int rc = scan_i64(d_count, n_pes, &total);
     if (rc != SB_OK) { release(); return rc; }
-    info[3] = misc[1] ? 1 : 0;
+    *cut = misc[1] ? 1 : 0;
     if (t->codec == SB_TS_PCM_BLURAY) {
         sbts::Lpcm f;
         if (sbts::parse_lpcm(misc[0], &f)) { release(); SB_FAIL(SB_EINVAL, "PID %d: no BD-LPCM header", t->pid); }
-        if (total > 0 && pool_alloc((void**)&t->d_pcm, sizeof(int16_t) * (size_t)(total * f.channels) + 16) != SB_OK) {
+        int16_t* d_pcm = nullptr;
+        if (total > 0 && pool_alloc((void**)&d_pcm, sizeof(int16_t) * (size_t)(total * f.channels) + 16) != SB_OK) {
             release();
             SB_FAIL(SB_ENOMEM, "sb_ts_finish: out of device memory for %lld sample frames", (long long)total);
         }
@@ -465,16 +461,13 @@ int sb_ts_finish(sb_ts* t, int32_t* info, int64_t* frames_out) {
             ProfScope ps("bdlpcm_decode");
             const int grid = (int)std::min<int64_t>((total + kThreads - 1) / kThreads, (int64_t)c.sm_count * 16);
             // the scan left each PES's first frame in d_count
-            k_bdlpcm_decode<<<grid, kThreads, 0, c.stream>>>(t->d_es, d_off, d_count, n_pes, total, f, t->d_pcm);
+            k_bdlpcm_decode<<<grid, kThreads, 0, c.stream>>>(t->d_es, d_off, d_count, n_pes, total, f, d_pcm);
             e = cudaGetLastError();
         }
         if (e == cudaSuccess) e = cudaStreamSynchronize(c.stream);
         release();
-        if (e != cudaSuccess) SB_FAIL(SB_ECUDA, "sb_ts_finish: %s", cudaGetErrorString(e));
-        t->frames = total; t->channels = f.channels; t->rate = f.rate;
-        info[0] = f.channels; info[1] = f.rate; info[2] = f.bits;
-        *frames_out = total;
-        return SB_OK;
+        if (e != cudaSuccess) { pool_free(d_pcm); SB_FAIL(SB_ECUDA, "sb_ts_finish: %s", cudaGetErrorString(e)); }
+        return pcm_handle(d_pcm, total, f.channels, f.rate, out);
     }
     // TrueHD: the kept payloads back to back, then the .thd decoder on them as one block
     if (total < 1) { release(); SB_FAIL(SB_EINVAL, "PID %d carries no TrueHD payload", t->pid); }
@@ -524,39 +517,16 @@ int sb_ts_finish(sb_ts* t, int32_t* info, int64_t* frames_out) {
         return k >= 0 ? tab[(size_t)k].file_off : -1;
     };
     const int64_t zero = 0;
-    int32_t thd_info[2] = {0, 0};
-    int64_t frames = 0;
-    rc = truehd_index_device(host.data(), d_thd, total, &zero, d_block, 1, where, thd_info, &t->thd, &frames);
+    rc = truehd_index_device(host.data(), d_thd, total, &zero, d_block, 1, where, out);
     release_thd();
-    if (rc != SB_OK) return rc;
-    t->frames = frames; t->channels = thd_info[0]; t->rate = thd_info[1];
-    info[0] = thd_info[0]; info[1] = thd_info[1]; info[2] = 24;
-    *frames_out = frames;
-    return SB_OK;
-}
-
-int sb_ts_decode(sb_ts* t, int sample_rate, int64_t padding, int64_t total_len, sb_stream** out_f32) {
-    Ctx& c = ctx();
-    if (!c.inited) SB_FAIL(SB_ESTATE, "sb_ts_decode: library not initialised (call sb_init)");
-    if (!t || !out_f32) SB_FAIL(SB_EINVAL, "sb_ts_decode: NULL argument");
-    if (!t->finished || (!t->d_pcm && !t->thd && t->frames)) SB_FAIL(SB_ESTATE, "sb_ts_decode: call sb_ts_finish first");
-    if (t->thd) return sb_truehd_decode(t->thd, sample_rate, padding, total_len, out_f32);
-    sb_stream* s = nullptr;
-    const int rc = load_pcm_device(reinterpret_cast<const unsigned char*>(t->d_pcm), t->frames, t->channels, 2, t->rate,
-                                   sample_rate, padding, total_len, &s, "sb_ts_decode");
-    const cudaError_t e = cudaStreamSynchronize(c.stream);
-    if (rc != SB_OK) return rc;
-    if (e != cudaSuccess) { sb_stream_destroy(s); SB_FAIL(SB_ECUDA, "sb_ts_decode: %s", cudaGetErrorString(e)); }
-    *out_f32 = s;
-    return SB_OK;
+    return rc;
 }
 
 int sb_ts_destroy(sb_ts* t) {
     if (!t) return SB_OK;
     if (t->pending) cudaEventSynchronize(t->done);
     t->release_demux();
-    pool_free(t->d_run); pool_free(t->d_err); pool_free(t->d_pcm);
-    if (t->thd) sb_truehd_destroy(t->thd);
+    pool_free(t->d_run); pool_free(t->d_err);
     if (t->h_run) cudaFreeHost(t->h_run);
     if (t->done) cudaEventDestroy(t->done);
     if (t->copied) cudaEventDestroy(t->copied);

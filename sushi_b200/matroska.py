@@ -14,7 +14,7 @@ is never read.  What comes out:
 
 A block cut short by the end of the file is dropped with a warning and everything before it loads; a size that runs
 past its parent, or a lace table that runs past its block, raises SushiError naming the byte offset.  Audio decoding
-is not here: WavStream hands a FLAC or PCM track's frames to the GPU (sb_flac_index_frames / sb_load_pcm).
+is not here: WavStream hands a FLAC or PCM track's frames to the GPU (sb_flac_decode_frames / sb_load_pcm).
 """
 import io
 import logging

@@ -1,6 +1,6 @@
 """Dolby TrueHD streams on the host: recognising a raw .thd file and reading its first major sync (sample rate, samples
 per access unit, substreams, the decoded presentation's channel count) for the refusals WavStream gives before the GPU
-is touched.  The decode itself, and every check of the stream, is sb_truehd_index on the GPU."""
+is touched.  The decode itself, and every check of the stream, is sb_truehd_decode on the GPU."""
 from .common import SushiError
 
 SYNC_TRUEHD = b'\xf8\x72\x6f\xba'

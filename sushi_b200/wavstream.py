@@ -84,6 +84,16 @@ class DownmixedWavFile(object):
             self.close()
             raise
 
+    @classmethod
+    def from_bytes(cls, data, channels, framerate, sample_width):
+        """A reader over in-memory interleaved little-endian PCM, as if it were a WAV file's data chunk."""
+        self = cls.__new__(cls)
+        self._file = io.BytesIO(data)
+        self.channels_count, self.framerate, self.sample_width = channels, framerate, sample_width
+        self.frame_size = channels * sample_width
+        self.frames_count = len(data) // self.frame_size
+        return self
+
     def __del__(self):
         self.close()
 
@@ -146,7 +156,7 @@ class FlacFile(object):
     """FLAC metadata reader: an optional leading ID3v2 tag, the marker, then the metadata blocks.  STREAMINFO (which
     must come first) gives the stream parameters; every other block (PADDING, APPLICATION, SEEKTABLE, VORBIS_COMMENT,
     CUESHEET, PICTURE) is skipped.  `frame_offset` is where the first audio frame starts; the frames are decoded on the
-    GPU (sb_flac_index / sb_flac_decode)."""
+    GPU (sb_flac_decode_file / sb_flac_decode_frames)."""
 
     def __init__(self, path):
         with open(path, 'rb') as f:
@@ -198,6 +208,37 @@ class FlacFile(object):
         if self.framerate < 1:
             raise SushiError('{0}: FLAC STREAMINFO sample rate is 0'.format(path))
         self.frame_offset = at
+
+    def check_depth(self):
+        """SushiError unless the samples have 16 or 24 bits, the depths the GPU decoder takes."""
+        if self.bits_per_sample not in (16, 24):
+            raise SushiError('FLAC with {0} bits per sample is not supported (16 or 24)'.format(self.bits_per_sample))
+
+
+_CODEC_NAMES = {'flac': 'FLAC', 'alac': 'ALAC', 'truehd': 'TrueHD', 'pcm_bluray': 'BD-LPCM'}
+
+
+def _refuse_host(path, codec, loader):
+    """Compressed inputs are decoded on the GPU only."""
+    if loader != 'gpu':
+        raise SushiError("{0}: {1} input needs loader='gpu' (there is no host {1} decoder)".format(path, codec))
+
+
+def _decode(lib, name, *args):
+    """The sb_pcm handle a decoder entry point returns through its last argument."""
+    h = ctypes.c_void_p()
+    with nvtx_range('sushi_b200: ' + name):
+        _native.check(getattr(lib, name)(*args, ctypes.byref(h)), name)
+    return h
+
+
+def _decode_frames(lib, name, data, offsets, blocks, *args):
+    """_decode of frames listed in `data`: frame f starts at offsets[f]; blocks[f] is the file offset errors name."""
+    buf = np.frombuffer(data + b'\0', dtype=np.uint8)          # never empty
+    offsets = np.ascontiguousarray(offsets, np.int64)
+    blocks = np.ascontiguousarray(blocks, np.int64)
+    return _decode(lib, name, buf.ctypes.data_as(ctypes.c_void_p), len(data) or 1, offsets.ctypes.data_as(_native.c_i64p),
+                   blocks.ctypes.data_as(_native.c_i64p), len(offsets), *args)
 
 
 def decode_downmix(raw, sample_width, channels):
@@ -325,25 +366,21 @@ class WavStream(StreamGeometry):
         self._handle = None
         before_read = time()
         if isinstance(path, mpegts.TransportStream) or mpegts.is_transport_stream(path):
-            self._load_ts(path, sample_rate, sample_type, device, loader, track)
-            logging.info('Done reading transport stream {0} in {1}s'.format(path, time() - before_read))
-            return
-        if isinstance(path, mp4.Mp4File) or (not isinstance(path, matroska.MatroskaFile) and mp4.is_mp4(path)):
-            self._load_mp4(path, sample_rate, sample_type, device, loader, track)
-            logging.info('Done reading MP4 {0} in {1}s'.format(path, time() - before_read))
-            return
-        if isinstance(path, matroska.MatroskaFile) or matroska.is_matroska(path):
-            self._load_matroska(path, sample_rate, sample_type, device, loader, track)
-            logging.info('Done reading Matroska {0} in {1}s'.format(path, time() - before_read))
-            return
-        if truehd.is_truehd(path):
-            self._load_truehd(path, sample_rate, sample_type, device, loader)
-            logging.info('Done reading TrueHD {0} in {1}s'.format(path, time() - before_read))
-            return
-        if is_flac(path):
-            self._load_flac(path, sample_rate, sample_type, device, loader)
-            logging.info('Done reading FLAC {0} in {1}s'.format(path, time() - before_read))
-            return
+            name, load = 'transport stream', self._load_ts
+        elif isinstance(path, mp4.Mp4File) or (not isinstance(path, matroska.MatroskaFile) and mp4.is_mp4(path)):
+            name, load = 'MP4', self._load_mp4
+        elif isinstance(path, matroska.MatroskaFile) or matroska.is_matroska(path):
+            name, load = 'Matroska', self._load_matroska
+        elif truehd.is_truehd(path):
+            name, load = 'TrueHD', self._load_truehd
+        elif is_flac(path):
+            name, load = 'FLAC', self._load_flac
+        else:
+            name, load = 'WAV', self._load_wav
+        load(path, sample_rate, sample_type, device, loader, track)
+        logging.info('Done reading {0} {1} in {2}s'.format(name, path, time() - before_read))
+
+    def _load_wav(self, path, sample_rate, sample_type, device, loader, track):
         stream = DownmixedWavFile(path)
         try:
             if loader == 'gpu':
@@ -362,283 +399,162 @@ class WavStream(StreamGeometry):
             raise SushiError('Error while loading {0}: {1}'.format(path, e))
         finally:
             stream.close()
-        logging.info('Done reading WAV {0} in {1}s'.format(path, time() - before_read))
 
-    def _load_flac(self, path, sample_rate, sample_type, device, loader):
-        """A FLAC file loads exactly as the plain PCM WAV of its decoded samples: the frames are decoded on the GPU
-        into the int16 PCM sb_load_pcm would read from that WAV (24-bit samples keep their top 16 bits), and the
-        rest is the WAV path.  There is no host decoder, so loader='host' is refused."""
+    def _load_flac(self, path, sample_rate, sample_type, device, loader, track):
+        """A FLAC file: its frames are found by their sync codes and decoded on the GPU (sb_flac_decode_file)."""
         flac = FlacFile(path)
-        if flac.bits_per_sample not in (16, 24):
-            raise SushiError('FLAC with {0} bits per sample is not supported (16 or 24)'.format(flac.bits_per_sample))
-        if loader != 'gpu':
-            raise SushiError("{0}: FLAC input needs loader='gpu' (there is no host FLAC decoder)".format(path))
+        flac.check_depth()
+        _refuse_host(path, 'FLAC', loader)
         lib = _native.lib(device)
-        h = ctypes.c_void_p()
-        frames = ctypes.c_int64()
         buf = np.frombuffer(flac.data, dtype=np.uint8)
-        with nvtx_range('sushi_b200: sb_flac_index'):
-            _native.check(lib.sb_flac_index(buf.ctypes.data_as(ctypes.c_void_p), len(flac.data), flac.frame_offset,
-                                            flac.channels_count, flac.bits_per_sample, flac.framerate,
-                                            ctypes.byref(h), ctypes.byref(frames)), 'sb_flac_index')
-        try:
-            def decode(padding, total):
-                raw = ctypes.c_void_p()
-                with nvtx_range('sushi_b200: sb_flac_decode'):
-                    _native.check(lib.sb_flac_decode(h, sample_rate, padding, total, ctypes.byref(raw)), 'sb_flac_decode')
-                # after the frames passed their checks, which name a damaged frame more precisely than the total does
-                if flac.total_samples and flac.total_samples != frames.value:
-                    lib.sb_stream_destroy(raw)
-                    raise SushiError('{0}: FLAC STREAMINFO says {1} samples, the frames hold {2}'.format(
-                        path, flac.total_samples, frames.value))
-                return raw
-            self._load_gpu_with(decode, frames.value, flac.framerate, sample_rate, sample_type, device)
-        finally:
-            lib.sb_flac_destroy(h)
+        h = _decode(lib, 'sb_flac_decode_file', buf.ctypes.data_as(ctypes.c_void_p), len(flac.data), flac.frame_offset,
+                    flac.channels_count, flac.bits_per_sample, flac.framerate)
 
-    def _load_truehd(self, path, sample_rate, sample_type, device, loader):
-        """A raw TrueHD stream loads exactly as the plain PCM WAV of the samples FFmpeg's decoder returns (their top 16
-        bits): one block holding every access unit, decoded on the GPU.  There is no host decoder."""
+        def check(frames):
+            # after the frames passed their checks, which name a damaged frame more precisely than the total does
+            if flac.total_samples and flac.total_samples != frames:
+                raise SushiError('{0}: FLAC STREAMINFO says {1} samples, the frames hold {2}'.format(
+                    path, flac.total_samples, frames))
+        self._load_decoded(h, sample_rate, sample_type, device, check)
+
+    def _load_truehd(self, path, sample_rate, sample_type, device, loader, track):
+        """A raw TrueHD stream: one block holding every access unit (sb_truehd_decode)."""
         data, _ = truehd.read_stream(path)
-        if loader != 'gpu':
-            raise SushiError("{0}: TrueHD input needs loader='gpu' (there is no host TrueHD decoder)".format(path))
+        _refuse_host(path, 'TrueHD', loader)
         # one block; a negative file offset makes messages name each access unit's own offset
-        self._load_truehd_blocks(data, np.zeros(1, np.int64), np.full(1, -1, np.int64), sample_rate, sample_type, device)
-
-    def _load_truehd_blocks(self, data, offsets, blocks, sample_rate, sample_type, device):
-        """sb_truehd_index on the stream's blocks (offsets into data; blocks: their file offsets), then the loader."""
-        lib = _native.lib(device)
-        h = ctypes.c_void_p()
-        n = ctypes.c_int64()
-        info = np.zeros(2, np.int32)
-        buf = np.frombuffer(data + b'\0', dtype=np.uint8)
-        offsets = np.ascontiguousarray(offsets, np.int64)
-        blocks = np.ascontiguousarray(blocks, np.int64)
-        with nvtx_range('sushi_b200: sb_truehd_index'):
-            _native.check(lib.sb_truehd_index(buf.ctypes.data_as(ctypes.c_void_p), len(data),
-                                              offsets.ctypes.data_as(_native.c_i64p), blocks.ctypes.data_as(_native.c_i64p),
-                                              len(offsets), info.ctypes.data_as(_native.c_i32p), ctypes.byref(h),
-                                              ctypes.byref(n)), 'sb_truehd_index')
-        try:
-            def decode(padding, total):
-                raw = ctypes.c_void_p()
-                with nvtx_range('sushi_b200: sb_truehd_decode'):
-                    _native.check(lib.sb_truehd_decode(h, sample_rate, padding, total, ctypes.byref(raw)),
-                                  'sb_truehd_decode')
-                return raw
-            self._load_gpu_with(decode, n.value, int(info[1]), sample_rate, sample_type, device)
-        finally:
-            lib.sb_truehd_destroy(h)
+        h = _decode_frames(_native.lib(device), 'sb_truehd_decode', data, np.zeros(1, np.int64), np.full(1, -1, np.int64))
+        self._load_decoded(h, sample_rate, sample_type, device)
 
     def _load_ts(self, path, sample_rate, sample_type, device, loader, track):
-        """A transport stream's BD-LPCM or TrueHD stream loads exactly as the plain PCM WAV of the samples FFmpeg's
-        decoder returns.  The file is read in chunks of mpegts.CHUNK_BYTES into two page-locked buffers, one after the
-        other, so that the GPU scans one chunk while the next is read; demuxing and decoding are sb_ts_* on the GPU.
-        There is no host decoder, so loader='host' is refused."""
+        """A transport stream's BD-LPCM or TrueHD stream (sb_ts_*).  The file is read in chunks of mpegts.CHUNK_BYTES
+        into two page-locked buffers, one after the other, so that the GPU scans one chunk while the next is read."""
         ts = path if isinstance(path, mpegts.TransportStream) else mpegts.TransportStream(path)
         s = ts.select('audio', track)
         kind = mpegts.audio_codec(s)
-        if loader != 'gpu':
-            raise SushiError("{0}: {1} input needs loader='gpu' (there is no host decoder)".format(
-                ts.path, 'TrueHD' if kind == 'truehd' else 'BD-LPCM'))
+        _refuse_host(ts.path, _CODEC_NAMES[kind], loader)
         lib = _native.lib(device)
-        h = ctypes.c_void_p()
+        t = ctypes.c_void_p()
         codec = _native.SB_TS_TRUEHD if kind == 'truehd' else _native.SB_TS_PCM_BLURAY
-        _native.check(lib.sb_ts_open(ts.packet_size, s.pid, codec, ctypes.byref(h)), 'sb_ts_open')
+        _native.check(lib.sb_ts_open(ts.packet_size, s.pid, codec, ctypes.byref(t)), 'sb_ts_open')
+        cut = ctypes.c_int32()
         try:
             size = max(ts.packet_size, mpegts.CHUNK_BYTES // ts.packet_size * ts.packet_size)
             buffers = [_native.pinned_empty((size,), np.uint8) for _ in range(2)]
             with nvtx_range('sushi_b200: sb_ts_feed'):
                 for view, pos in ts.chunks(buffers):
                     arr = np.frombuffer(view, np.uint8)
-                    _native.check(lib.sb_ts_feed(h, arr.ctypes.data_as(ctypes.c_void_p), len(arr), pos), 'sb_ts_feed')
+                    _native.check(lib.sb_ts_feed(t, arr.ctypes.data_as(ctypes.c_void_p), len(arr), pos), 'sb_ts_feed')
             del buffers
-            info = np.zeros(4, np.int32)
-            n = ctypes.c_int64()
-            with nvtx_range('sushi_b200: sb_ts_finish'):
-                _native.check(lib.sb_ts_finish(h, info.ctypes.data_as(_native.c_i32p), ctypes.byref(n)), 'sb_ts_finish')
-            if info[3]:
-                logging.warning('{0}: the last PES packet of stream {1} is cut short; its whole sample frames are '
-                                'kept'.format(ts.path, s.id))
-
-            def decode(padding, total):
-                raw = ctypes.c_void_p()
-                with nvtx_range('sushi_b200: sb_ts_decode'):
-                    _native.check(lib.sb_ts_decode(h, sample_rate, padding, total, ctypes.byref(raw)), 'sb_ts_decode')
-                return raw
-            self._load_gpu_with(decode, n.value, int(info[1]), sample_rate, sample_type, device)
+            h = _decode(lib, 'sb_ts_finish', t, ctypes.byref(cut))
         finally:
-            lib.sb_ts_destroy(h)
+            lib.sb_ts_destroy(t)
+        if cut.value:
+            logging.warning('{0}: the last PES packet of stream {1} is cut short; its whole sample frames are '
+                            'kept'.format(ts.path, s.id))
+        self._load_decoded(h, sample_rate, sample_type, device)
 
     def _load_matroska(self, path, sample_rate, sample_type, device, loader, track):
-        """A Matroska audio track loads exactly as the plain PCM WAV of its decoded samples, frames concatenated in
-        block order (timestamp gaps are not filled).  FLAC frames are decoded on the GPU where the container lists
-        them (sb_flac_index_frames; a cut track's frame numbers and stale STREAMINFO total are not checked);
-        little-endian PCM is a WAV data chunk as it stands and goes through sb_load_pcm.  `path` is a file name or an
-        opened MatroskaFile (left open; the track's table is released from it)."""
+        """A Matroska audio track (_load_track; a FLAC track's frame numbers and stale STREAMINFO total are not
+        checked).  `path` is a file name or an opened MatroskaFile (left open; the track's table is released from
+        it)."""
         opened = isinstance(path, matroska.MatroskaFile)
         mkv = path if opened else matroska.MatroskaFile(path)
-        path = mkv.path
         try:
             t = mkv.select('audio', track)
             kind = matroska.audio_codec(t)
-            if kind == 'flac':
-                info = FlacFile.from_bytes(t.codec_private, '{0} track {1}'.format(path, t.id))
-                if info.bits_per_sample not in (16, 24):
-                    raise SushiError('FLAC with {0} bits per sample is not supported (16 or 24)'.format(
-                        info.bits_per_sample))
-                if loader != 'gpu':
-                    raise SushiError("{0}: FLAC input needs loader='gpu' (there is no host FLAC decoder)".format(path))
-            if kind == 'truehd' and loader != 'gpu':
-                raise SushiError("{0}: TrueHD input needs loader='gpu' (there is no host TrueHD decoder)".format(path))
-            if kind == 'alac' and loader != 'gpu':
-                raise SushiError("{0}: ALAC input needs loader='gpu' (there is no host ALAC decoder)".format(path))
-            table = mkv.frames([t.id])[t.id]
-            mkv.release([t.id])
+
+            def read_frames():
+                table = mkv.frames([t.id])[t.id]
+                mkv.release([t.id])
+                return table
+            pcm = (t.channels, int(t.sampling_frequency), t.bit_depth // 8, False) if kind == 'pcm' else None
+            self._load_track(mkv.path, t.id, kind, t.codec_private, pcm, read_frames, sample_rate, sample_type, device,
+                             loader)
         finally:
             if not opened:
                 mkv.close()
-        if kind == 'flac':
-            table.refuse_empty(path, 'FLAC')
-        if kind == 'alac':
-            table.refuse_empty(path, 'ALAC')
-            self._load_alac_frames(table, t.codec_private[:24], sample_rate, sample_type, device)
-            return
-        if kind == 'truehd':
-            table.refuse_empty(path, 'TrueHD')
-            truehd.MajorSync(table.data[:64], '{0} track {1}'.format(path, t.id))
-            self._load_truehd_blocks(table.data, table.offset, table.block, sample_rate, sample_type, device)
-            return
-        if kind == 'pcm':
-            width = t.bit_depth // 8
-            frames = len(table.data) // (t.channels * width)
-            rate = int(t.sampling_frequency)
-            if loader == 'gpu':
-                self._load_gpu(table.data, frames, t.channels, width, rate, sample_rate, sample_type, device)
-            else:
-                mem = DownmixedWavFile.__new__(DownmixedWavFile)
-                mem._file = io.BytesIO(table.data)
-                mem.channels_count, mem.framerate, mem.sample_width = t.channels, rate, width
-                mem.frame_size, mem.frames_count = t.channels * width, frames
-                self._load(mem, sample_rate, sample_type)
-                self._upload(device)
-            return
-        self._load_flac_frames(table, info, sample_rate, sample_type, device)
-
-    def _load_flac_frames(self, table, info, sample_rate, sample_type, device):
-        """sb_flac_index_frames on a container's FLAC frames (table.block: each frame's file offset), then the loader."""
-        lib = _native.lib(device)
-        h = ctypes.c_void_p()
-        n = ctypes.c_int64()
-        buf = np.frombuffer(table.data + b'\0', dtype=np.uint8)          # never empty
-        offsets = np.ascontiguousarray(table.offset, np.int64)
-        blocks = np.ascontiguousarray(table.block, np.int64)
-        with nvtx_range('sushi_b200: sb_flac_index_frames'):
-            _native.check(lib.sb_flac_index_frames(buf.ctypes.data_as(ctypes.c_void_p), len(table.data) or 1,
-                                                   offsets.ctypes.data_as(_native.c_i64p),
-                                                   blocks.ctypes.data_as(_native.c_i64p), len(offsets),
-                                                   info.channels_count, info.bits_per_sample, info.framerate,
-                                                   ctypes.byref(h), ctypes.byref(n)), 'sb_flac_index_frames')
-        try:
-            def decode(padding, total):
-                raw = ctypes.c_void_p()
-                with nvtx_range('sushi_b200: sb_flac_decode'):
-                    _native.check(lib.sb_flac_decode(h, sample_rate, padding, total, ctypes.byref(raw)), 'sb_flac_decode')
-                return raw
-            self._load_gpu_with(decode, n.value, info.framerate, sample_rate, sample_type, device)
-        finally:
-            lib.sb_flac_destroy(h)
-
-    def _load_alac_frames(self, table, cookie, sample_rate, sample_type, device):
-        """sb_alac_index_frames on a container's ALAC frames (cookie: the 24-byte ALACSpecificConfig; table.block:
-        each frame's file offset, which errors name), then the loader."""
-        fl, _, depth, pb, mb, kb, channels, _, _, _, rate = struct.unpack('>IBBBBBBHIII', cookie)
-        config = np.array([fl, depth, pb, mb, kb, channels, rate], np.int32)
-        lib = _native.lib(device)
-        h = ctypes.c_void_p()
-        n = ctypes.c_int64()
-        buf = np.frombuffer(table.data + b'\0', dtype=np.uint8)
-        offsets = np.ascontiguousarray(table.offset, np.int64)
-        blocks = np.ascontiguousarray(table.block, np.int64)
-        with nvtx_range('sushi_b200: sb_alac_index_frames'):
-            _native.check(lib.sb_alac_index_frames(buf.ctypes.data_as(ctypes.c_void_p), len(table.data) or 1,
-                                                   offsets.ctypes.data_as(_native.c_i64p),
-                                                   blocks.ctypes.data_as(_native.c_i64p), len(offsets),
-                                                   config.ctypes.data_as(_native.c_i32p), ctypes.byref(h),
-                                                   ctypes.byref(n)), 'sb_alac_index_frames')
-        try:
-            def decode(padding, total):
-                raw = ctypes.c_void_p()
-                with nvtx_range('sushi_b200: sb_alac_decode'):
-                    _native.check(lib.sb_alac_decode(h, sample_rate, padding, total, ctypes.byref(raw)), 'sb_alac_decode')
-                return raw
-            self._load_gpu_with(decode, n.value, rate, sample_rate, sample_type, device)
-        finally:
-            lib.sb_alac_destroy(h)
 
     def _load_mp4(self, path, sample_rate, sample_type, device, loader, track):
-        """An MP4 / QuickTime audio track loads exactly as the plain PCM WAV of the samples FFmpeg's decoder returns.
-        ALAC and FLAC samples are decoded on the GPU where the sample table puts them; 16- and 24-bit PCM goes through
-        sb_load_pcm (little-endian) or sb_load_pcm_be (big-endian).  loader='host' works for PCM only.  `path` is a file
-        name or an opened Mp4File (left open)."""
+        """An MP4 / QuickTime audio track (_load_track).  `path` is a file name or an opened Mp4File (left open)."""
         opened = isinstance(path, mp4.Mp4File)
         f = path if opened else mp4.Mp4File(path)
-        path = f.path
         try:
             t = f.select('audio', track)
             kind = mp4.audio_codec(t)
             f.check_edits(t)
-            if kind == 'flac':
-                info = FlacFile.from_bytes(t.config, '{0} track {1}'.format(path, t.id))
-                if info.bits_per_sample not in (16, 24):
-                    raise SushiError('FLAC with {0} bits per sample is not supported (16 or 24)'.format(
-                        info.bits_per_sample))
-            if kind != 'pcm' and loader != 'gpu':
-                raise SushiError("{0}: {1} input needs loader='gpu' (there is no host {1} decoder)".format(
-                    path, kind.upper()))
-            table = f.frames(t)
+            pcm = (t.channels, t.rate) + mp4.PCM_DECODED[t.codec] if kind == 'pcm' else None
+            self._load_track(f.path, t.id, kind, t.config, pcm, lambda: f.frames(t), sample_rate, sample_type, device,
+                             loader)
         finally:
             if not opened:
                 f.close()
-        if kind == 'alac':
-            table.refuse_empty(path, 'ALAC')
-            self._load_alac_frames(table, t.config, sample_rate, sample_type, device)
-            return
+
+    def _load_track(self, path, track_id, kind, config, pcm, read_frames, sample_rate, sample_type, device, loader):
+        """A container's audio track loads exactly as the plain PCM WAV of the samples FFmpeg's decoder returns, frames
+        concatenated in container order (timestamp gaps are not filled).  `kind` is 'flac', 'alac', 'truehd' or 'pcm';
+        `config` the codec's configuration (FLAC metadata blocks, the ALACSpecificConfig); `pcm` (channels, rate,
+        sample width, big-endian) for PCM.  read_frames() reads the track's FrameTable, only once every refusal has
+        passed.  FLAC, ALAC and TrueHD frames are decoded on the GPU where the table puts them, errors naming the file
+        offset of a frame's block; PCM goes through sb_load_pcm (little-endian), sb_pcm_from_be (big-endian) or, for
+        loader='host', the host loader."""
+        name = '{0} track {1}'.format(path, track_id)
         if kind == 'flac':
-            table.refuse_empty(path, 'FLAC')
-            self._load_flac_frames(table, info, sample_rate, sample_type, device)
-            return
-        width, big = mp4.PCM_DECODED[t.codec]
-        frames = len(table.data) // (t.channels * width)
-        data = table.data[:frames * t.channels * width]
-        if loader == 'gpu':
-            if big:
-                self._load_gpu_be(data, frames, t.channels, width, t.rate, sample_rate, sample_type, device)
+            info = FlacFile.from_bytes(config, name)
+            info.check_depth()
+        if kind != 'pcm':
+            _refuse_host(path, _CODEC_NAMES[kind], loader)
+        table = read_frames()
+        if kind == 'pcm':
+            channels, rate, width, big = pcm
+            frames = len(table.data) // (channels * width)
+            data = table.data[:frames * channels * width]
+            if loader != 'gpu':
+                if big:
+                    data = np.frombuffer(data, np.uint8).reshape(-1, width)[:, ::-1].tobytes()
+                self._load(DownmixedWavFile.from_bytes(data, channels, rate, width), sample_rate, sample_type)
+                self._upload(device)
+            elif big:
+                buf = np.frombuffer(data, dtype=np.uint8)
+                h = _decode(_native.lib(device), 'sb_pcm_from_be', buf.ctypes.data_as(ctypes.c_void_p), frames, channels,
+                            width, rate)
+                self._load_decoded(h, sample_rate, sample_type, device)
             else:
-                self._load_gpu(data, frames, t.channels, width, t.rate, sample_rate, sample_type, device)
+                self._load_gpu(data, frames, channels, width, rate, sample_rate, sample_type, device)
             return
-        if big:
-            data = np.frombuffer(data, np.uint8).reshape(-1, width)[:, ::-1].tobytes()
-        mem = DownmixedWavFile.__new__(DownmixedWavFile)
-        mem._file = io.BytesIO(data)
-        mem.channels_count, mem.framerate, mem.sample_width = t.channels, t.rate, width
-        mem.frame_size, mem.frames_count = t.channels * width, frames
-        self._load(mem, sample_rate, sample_type)
-        self._upload(device)
-
-    def _load_gpu_be(self, pcm, frames, channels, sample_width, framerate, sample_rate, sample_type, device):
-        """_load_gpu for big-endian PCM: sb_load_pcm_be."""
-        buf = np.frombuffer(pcm, dtype=np.uint8, count=frames * channels * sample_width)
+        table.refuse_empty(path, _CODEC_NAMES[kind])
         lib = _native.lib(device)
+        if kind == 'flac':
+            h = _decode_frames(lib, 'sb_flac_decode_frames', table.data, table.offset, table.block, info.channels_count,
+                               info.bits_per_sample, info.framerate)
+        elif kind == 'alac':
+            fl, _, depth, pb, mb, kb, channels, _, _, _, rate = struct.unpack('>IBBBBBBHIII', config[:24])
+            cfg = np.array([fl, depth, pb, mb, kb, channels, rate], np.int32)
+            h = _decode_frames(lib, 'sb_alac_decode_frames', table.data, table.offset, table.block,
+                               cfg.ctypes.data_as(_native.c_i32p))
+        else:
+            truehd.MajorSync(table.data[:64], name)
+            h = _decode_frames(lib, 'sb_truehd_decode', table.data, table.offset, table.block)
+        self._load_decoded(h, sample_rate, sample_type, device)
 
-        def load(padding, total):
-            raw = ctypes.c_void_p()
-            with nvtx_range('sushi_b200: sb_load_pcm_be'):
-                _native.check(lib.sb_load_pcm_be(buf.ctypes.data_as(ctypes.c_void_p), frames, channels, sample_width,
-                                                 framerate, sample_rate, padding, total, ctypes.byref(raw)),
-                              'sb_load_pcm_be')
-            return raw
-        self._load_gpu_with(load, frames, framerate, sample_rate, sample_type, device)
+    def _load_decoded(self, h, sample_rate, sample_type, device, check=None):
+        """_load_gpu_with on a decoder's sb_pcm handle `h` (sb_pcm_load), which it destroys; check(frames) may refuse
+        the decoded frame count first."""
+        lib = _native.lib(device)
+        try:
+            frames, channels, rate = ctypes.c_int64(), ctypes.c_int32(), ctypes.c_int32()
+            _native.check(lib.sb_pcm_info(h, ctypes.byref(frames), ctypes.byref(channels), ctypes.byref(rate)),
+                          'sb_pcm_info')
+            if check is not None:
+                check(frames.value)
+
+            def load(padding, total):
+                raw = ctypes.c_void_p()
+                with nvtx_range('sushi_b200: sb_pcm_load'):
+                    _native.check(lib.sb_pcm_load(h, sample_rate, padding, total, ctypes.byref(raw)), 'sb_pcm_load')
+                return raw
+            self._load_gpu_with(load, frames.value, rate.value, sample_rate, sample_type, device)
+        finally:
+            lib.sb_pcm_destroy(h)
 
     def _load_gpu(self, pcm, frames, channels, sample_width, framerate, sample_rate, sample_type, device):
         """wav.py:108-156 on the GPU: geometry here (same scalar code as the reference), arithmetic
@@ -661,7 +577,7 @@ class WavStream(StreamGeometry):
 
     def _load_gpu_with(self, load, frames, framerate, sample_rate, sample_type, device):
         """The geometry of wav.py:113-120 for `frames` frames at `framerate`, then load(padding, total) -> the raw
-        float32 stream (sb_load_pcm or sb_flac_decode), normalised by sb_normalise and mirrored back."""
+        float32 stream (sb_load_pcm or sb_pcm_load), normalised by sb_normalise and mirrored back."""
         total_seconds = frames / float(framerate)
         self.sample_count = math.ceil(total_seconds * sample_rate)
         self.sample_rate = sample_rate
@@ -725,36 +641,17 @@ class WavStream(StreamGeometry):
     def from_pcm(cls, pcm, framerate, sample_rate=12000, sample_type='uint8', channels=1, device=None, loader='gpu'):
         """Build a stream from an in-memory int16 array (frames x channels, interleaved) --
         the same pipeline as a file load without the RIFF walk (synthetic benches/tests)."""
-        class _Mem(object):
-            pass
         pcm = np.ascontiguousarray(pcm, dtype='<i2')
         if sample_type not in _DTYPES:
             raise SushiError('Unknown sample type of WAV stream, must be uint8 or float32')
-        if loader == 'gpu':
-            self = object.__new__(cls)
-            self._handle = None
-            self._load_gpu(pcm.reshape(-1).view(np.uint8).tobytes(), pcm.size // channels, channels, 2,
-                           framerate, sample_rate, sample_type, device)
-            return self
-        mem = _Mem()
-        mem.framerate, mem.channels_count, mem.sample_width = framerate, channels, 2
-        mem.frame_size = 2 * channels
-        mem.frames_count = pcm.size // channels
-        raw = pcm.reshape(-1).view(np.uint8)
-        state = {'pos': 0}
-
-        def readframes(count):
-            a = state['pos']
-            b = min(a + count * mem.frame_size, raw.size)
-            state['pos'] = b
-            return decode_downmix(raw[a:b].tobytes(), 2, channels)
-        mem.readframes = readframes
         self = object.__new__(cls)
         self._handle = None
-        if sample_type not in _DTYPES:
-            raise SushiError('Unknown sample type of WAV stream, must be uint8 or float32')
-        self._load(mem, sample_rate, sample_type)
-        self._upload(device)
+        raw = pcm.reshape(-1).view(np.uint8).tobytes()
+        if loader == 'gpu':
+            self._load_gpu(raw, pcm.size // channels, channels, 2, framerate, sample_rate, sample_type, device)
+        else:
+            self._load(DownmixedWavFile.from_bytes(raw, channels, framerate, 2), sample_rate, sample_type)
+            self._upload(device)
         return self
 
     @classmethod

@@ -1,8 +1,8 @@
 // CPU build of the listed-frame path of the FLAC decoder: sushi_b200/csrc/sb_flac.cuh compiled with g++, driven the way
-// sb_flac_index_frames and sb_flac_decode drive it (tests/test_kernel_emulation_mkv_flac.py).  Each listed frame's
+// sb_flac_decode_frames drives it (tests/test_kernel_emulation_mkv_flac.py).  Each listed frame's
 // header is checked at its offset (k_flac_frames), the frame table is built from the block sizes, every frame is
 // decoded and checked against its lace end (k_flac_decode), and the channels are decorrelated (k_flac_decorrelate).
-// For comparison, emu_flac_chain_table builds the table sb_flac_index builds from a whole FLAC file.
+// For comparison, emu_flac_chain_table builds the table sb_flac_decode_file builds from a whole FLAC file.
 #include <stdint.h>
 #include <string.h>
 #include <vector>
@@ -41,7 +41,7 @@ int64_t emu_flac_frames(const uint8_t* buf, int64_t nbytes, const int64_t* offse
     return samples;
 }
 
-// sb_flac_index's chained table of a whole FLAC file (frames found by their sync codes and coded numbers).  Returns
+// sb_flac_decode_file's chained table of a whole FLAC file (frames found by their sync codes and coded numbers).  Returns
 // the frame count (table filled when it fits in `cap` frames), or -1 with the message in msg.
 int64_t emu_flac_chain_table(const uint8_t* file, int64_t nbytes, int64_t first, int channels, int bits, int rate,
                              int64_t* table, int64_t cap, char* msg, int msg_len) {

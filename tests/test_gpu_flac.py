@@ -1,4 +1,4 @@
-"""FLAC input on the GPU (sb_flac_index / sb_flac_decode behind WavStream(path)): a FLAC file loads bit for bit as the
+"""FLAC input on the GPU (sb_flac_decode_file / sb_pcm_load behind WavStream(path)): a FLAC file loads bit for bit as the
 plain PCM WAV of the same samples loads -- .data, sample_count, padding_size, sample_rate and both clip values -- on
 every case of tests/flac_cases.py in both sample types; damaged files raise SushiError naming the frame; the shift
 solver and the command line give the same script on a FLAC pair as on the WAV pair; and a BASELINE-size file (90

@@ -1,4 +1,4 @@
-"""Matroska input on the GPU (WavStream(path, track=...) over sb_flac_index_frames / sb_flac_decode and sb_load_pcm):
+"""Matroska input on the GPU (WavStream(path, track=...) over sb_flac_decode_frames / sb_pcm_load and sb_load_pcm):
 every audio track of tests/mkv_cases.py loads bit for bit as the plain PCM WAV of its samples loads -- .data,
 sample_count, padding_size, sample_rate and both clip values -- in both sample types, the cut FLAC track and each
 track of the multi-track file included; damaged FLAC frames raise SushiError naming their block's file offset; the

@@ -1,6 +1,6 @@
 """MP4 / QuickTime and A_ALAC Matroska inputs on the GPU: every audio track loads bit for bit as the plain PCM WAV of
 the samples FFmpeg's decoder returns (tests/test_mp4_cases.py and tests/test_alac_cases.py hold FFmpeg to the
-writers' PCM): ALAC through sb_alac_*, FLAC through sb_flac_index_frames, PCM through sb_load_pcm or sb_load_pcm_be.
+writers' PCM): ALAC through sb_alac_decode_frames, FLAC through sb_flac_decode_frames, PCM through sb_load_pcm or sb_pcm_from_be.
 Also 90 minutes of 24-bit stereo ALAC, the sparse file past 4 GiB, damaged frames named by frame and offset, and the
 command line against the WAV pair."""
 import os

@@ -1,4 +1,4 @@
-"""TrueHD input on the GPU (sb_truehd_index / sb_truehd_decode behind WavStream): a raw .thd stream and a Matroska
+"""TrueHD input on the GPU (sb_truehd_decode / sb_pcm_load behind WavStream): a raw .thd stream and a Matroska
 A_TRUEHD track load bit for bit as the plain PCM WAV of the samples FFmpeg's decoder returns (tests/test_truehd_cases.py
 holds FFmpeg to the writer's PCM) -- .data, sample_count, padding_size, sample_rate and both clip values -- in both
 sample types; each damaged stream raises SushiError naming the access unit and its byte offset; the shift solver and

@@ -1,8 +1,8 @@
-"""The listed-frame path of the FLAC decoder (k_flac_frames' per-frame logic and the table sb_flac_index_frames builds,
+"""The listed-frame path of the FLAC decoder (k_flac_frames' per-frame logic and the table sb_flac_decode_frames builds,
 from sushi_b200/csrc/sb_flac.cuh) on the CPU, through tests/emu/emu_flac_frames_driver.cpp compiled with g++:
 
 * listing every frame of every uncut FLAC case of tests/flac_cases.py at its offset builds the same frame table as the
-  sync-code chain of sb_flac_index;
+  sync-code chain of sb_flac_decode_file;
 * every FLAC track of tests/mkv_cases.py decodes bit for bit to its PCM, the cut track (frame numbers from 5, a stale
   STREAMINFO total) included;
 * a frame with a bad CRC-8 or CRC-16 is named with the file offset of the block holding it."""
