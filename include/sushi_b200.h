@@ -39,7 +39,7 @@
 extern "C" {
 #endif
 
-#define SB_ABI_VERSION 9
+#define SB_ABI_VERSION 10
 
 /* status codes */
 #define SB_OK            0
@@ -281,6 +281,21 @@ int sb_truehd_decode(const void* buf, int64_t nbytes, const int64_t* offsets, co
  * header; a frame that reads past its bytes; a frame without END.  Bytes after END are ignored. */
 int sb_alac_decode_frames(const void* buf, int64_t nbytes, const int64_t* offsets, const int64_t* file_offsets, int64_t n,
                           const int32_t* config, sb_pcm** out);
+
+/* WavPack (ABI version 10): FFmpeg's `wavpack` decoder output for lossless integer streams of 2 or 3 bytes per sample,
+ * 3-byte samples by the top 16 bits of FFmpeg's S32 sample, channels in FFmpeg's order (blocks in order within a
+ * frame).  `buf` holds the stream's blocks (`nbytes` bytes); table holds 8 int64 per block b: the offset and size of
+ * its metadata sub-blocks in buf, block_samples (1 to 150000), the header's flags and CRC, the track sample where the
+ * block starts, its first output channel (a block fills one channel when its flags say mono, two otherwise), and the
+ * byte offset in the file of the block's header (.wv) or Matroska block, which every error names with the block index.
+ * The host builds the table from the block headers and checks their sequence; `channels` (1 to 8) and `rate` are the
+ * stream's.  One GPU thread decodes each block.  It fails on: hybrid, float, DSD or 1- / 4-byte flags; a sub-block
+ * that runs past its block; samples without ID_WV_BITSTREAM, or without terms, weights, sample history or medians;
+ * more than 16 decorrelation terms or an invalid one; invalid weights, sample history, medians, ID_INT32_INFO or
+ * ID_SAMPLE_RATE; extended precision (ID_WVX_BITSTREAM, ID_INT32_INFO sent bits); a mono block without terms; a
+ * bitstream that reads past its sub-block; a 16-bit stereo sample above 2^19; a block CRC that disagrees. */
+int sb_wavpack_decode_blocks(const void* buf, int64_t nbytes, const int64_t* table, int64_t n, int32_t channels,
+                             int32_t rate, sb_pcm** out);
 
 /* ---- MPEG transport streams (ABI version 7) ----------------------------------
  *

@@ -24,6 +24,7 @@ import zlib
 
 import numpy as np
 
+from . import wavpack
 from .common import SushiError, py2_round, select_stream
 
 EBML_MAGIC = b'\x1a\x45\xdf\xa3'
@@ -684,8 +685,9 @@ class MatroskaFile(object):
 
 
 def audio_codec(track):
-    """'flac', 'truehd', 'alac' or 'pcm' for an audio track the GPU loader decodes (FLAC, Dolby TrueHD, ALAC, whose
-    CodecPrivate is the ALACSpecificConfig, little-endian integer PCM of 16 or 24 bits);
+    """'flac', 'truehd', 'alac', 'wavpack' or 'pcm' for an audio track the GPU loader decodes (FLAC, Dolby TrueHD, ALAC,
+    whose CodecPrivate is the ALACSpecificConfig, WavPack stream versions 0x402-0x410, little-endian integer PCM of 16
+    or 24 bits);
     SushiError naming the track and its codec for anything else."""
     if track.refusal:
         raise SushiError(track.refusal)
@@ -697,8 +699,11 @@ def audio_codec(track):
         return 'alac'
     if track.codec_id == 'A_PCM/INT/LIT' and track.bit_depth in (16, 24) and track.channels >= 1:
         return 'pcm'
+    if track.codec_id == 'A_WAVPACK4':
+        wavpack.check_version(track.codec_private, track.id)
+        return 'wavpack'
     what = track.codec_id + (' at {0} bits'.format(track.bit_depth) if track.codec_id.startswith('A_PCM') else '')
-    raise SushiError('Audio track {0} is {1}, which cannot be decoded here (FLAC, TrueHD, ALAC and 16- or '
+    raise SushiError('Audio track {0} is {1}, which cannot be decoded here (FLAC, TrueHD, ALAC, WavPack and 16- or '
                      '24-bit little-endian PCM can): convert it to FLAC or WAV first'.format(track.id, what))
 
 

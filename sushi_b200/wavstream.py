@@ -24,7 +24,7 @@ from time import time
 
 import numpy as np
 
-from . import _native, matroska, mp4, mpegts, truehd
+from . import _native, matroska, mp4, mpegts, truehd, wavpack
 from ._nvtx import nvtx_range
 from .common import SushiError, clip, py2_round
 
@@ -215,7 +215,7 @@ class FlacFile(object):
             raise SushiError('FLAC with {0} bits per sample is not supported (16 or 24)'.format(self.bits_per_sample))
 
 
-_CODEC_NAMES = {'flac': 'FLAC', 'alac': 'ALAC', 'truehd': 'TrueHD', 'pcm_bluray': 'BD-LPCM'}
+_CODEC_NAMES = {'flac': 'FLAC', 'alac': 'ALAC', 'truehd': 'TrueHD', 'pcm_bluray': 'BD-LPCM', 'wavpack': 'WavPack'}
 
 
 def _refuse_host(path, codec, loader):
@@ -239,6 +239,14 @@ def _decode_frames(lib, name, data, offsets, blocks, *args):
     blocks = np.ascontiguousarray(blocks, np.int64)
     return _decode(lib, name, buf.ctypes.data_as(ctypes.c_void_p), len(data) or 1, offsets.ctypes.data_as(_native.c_i64p),
                    blocks.ctypes.data_as(_native.c_i64p), len(offsets), *args)
+
+
+def _decode_blocks(lib, data, table, stream):
+    """_decode of sb_wavpack_decode_blocks on the blocks of `table` (wavpack's 8-column block table) in `data`"""
+    buf = np.frombuffer(data, dtype=np.uint8)
+    table = np.ascontiguousarray(table, np.int64)
+    return _decode(lib, 'sb_wavpack_decode_blocks', buf.ctypes.data_as(ctypes.c_void_p), len(data),
+                   table.ctypes.data_as(_native.c_i64p), len(table), stream.channels, stream.rate)
 
 
 def decode_downmix(raw, sample_width, channels):
@@ -373,6 +381,8 @@ class WavStream(StreamGeometry):
             name, load = 'Matroska', self._load_matroska
         elif truehd.is_truehd(path):
             name, load = 'TrueHD', self._load_truehd
+        elif wavpack.is_wavpack(path):
+            name, load = 'WavPack', self._load_wavpack
         elif is_flac(path):
             name, load = 'FLAC', self._load_flac
         else:
@@ -425,6 +435,14 @@ class WavStream(StreamGeometry):
         h = _decode_frames(_native.lib(device), 'sb_truehd_decode', data, np.zeros(1, np.int64), np.full(1, -1, np.int64))
         self._load_decoded(h, sample_rate, sample_type, device)
 
+    def _load_wavpack(self, path, sample_rate, sample_type, device, loader, track):
+        """A raw WavPack (.wv) file: its block chain walked on the host (wavpack.WavPackFile, which refuses what cannot
+        be decoded and a broken chain), every block decoded on the GPU (sb_wavpack_decode_blocks)."""
+        f = wavpack.WavPackFile(path)
+        _refuse_host(path, 'WavPack', loader)
+        self._load_decoded(_decode_blocks(_native.lib(device), f.data, f.table, f.stream), sample_rate, sample_type,
+                           device)
+
     def _load_ts(self, path, sample_rate, sample_type, device, loader, track):
         """A transport stream's BD-LPCM or TrueHD stream (sb_ts_*).  The file is read in chunks of mpegts.CHUNK_BYTES
         into two page-locked buffers, one after the other, so that the GPU scans one chunk while the next is read."""
@@ -468,7 +486,9 @@ class WavStream(StreamGeometry):
                 mkv.release([t.id])
                 return table
             pcm = (t.channels, int(t.sampling_frequency), t.bit_depth // 8, False) if kind == 'pcm' else None
-            self._load_track(mkv.path, t.id, kind, t.codec_private, pcm, read_frames, sample_rate, sample_type, device,
+            # WavPack: the stream version, and the channel count a multi-block frame must code
+            config = (t.codec_private, t.channels) if kind == 'wavpack' else t.codec_private
+            self._load_track(mkv.path, t.id, kind, config, pcm, read_frames, sample_rate, sample_type, device,
                              loader)
         finally:
             if not opened:
@@ -491,11 +511,11 @@ class WavStream(StreamGeometry):
 
     def _load_track(self, path, track_id, kind, config, pcm, read_frames, sample_rate, sample_type, device, loader):
         """A container's audio track loads exactly as the plain PCM WAV of the samples FFmpeg's decoder returns, frames
-        concatenated in container order (timestamp gaps are not filled).  `kind` is 'flac', 'alac', 'truehd' or 'pcm';
-        `config` the codec's configuration (FLAC metadata blocks, the ALACSpecificConfig); `pcm` (channels, rate,
-        sample width, big-endian) for PCM.  read_frames() reads the track's FrameTable, only once every refusal has
-        passed.  FLAC, ALAC and TrueHD frames are decoded on the GPU where the table puts them, errors naming the file
-        offset of a frame's block; PCM goes through sb_load_pcm (little-endian), sb_pcm_from_be (big-endian) or, for
+        concatenated in container order (timestamp gaps are not filled).  `kind` is 'flac', 'alac', 'truehd', 'wavpack'
+        or 'pcm'; `config` the codec's configuration (FLAC metadata blocks, the ALACSpecificConfig, WavPack's
+        (CodecPrivate, channel count)); `pcm` (channels, rate, sample width, big-endian) for PCM.  read_frames() reads
+        the track's FrameTable, only once every refusal has passed.  FLAC, ALAC, WavPack and TrueHD frames are
+        decoded on the GPU where the table puts them, errors naming the file offset of a frame's block; PCM goes through sb_load_pcm (little-endian), sb_pcm_from_be (big-endian) or, for
         loader='host', the host loader."""
         name = '{0} track {1}'.format(path, track_id)
         if kind == 'flac':
@@ -522,10 +542,14 @@ class WavStream(StreamGeometry):
                 self._load_gpu(data, frames, channels, width, rate, sample_rate, sample_type, device)
             return
         table.refuse_empty(path, _CODEC_NAMES[kind])
+        if kind == 'wavpack':
+            blocks, stream = wavpack.matroska_table(table, config[0], track_id, config[1])
         lib = _native.lib(device)
         if kind == 'flac':
             h = _decode_frames(lib, 'sb_flac_decode_frames', table.data, table.offset, table.block, info.channels_count,
                                info.bits_per_sample, info.framerate)
+        elif kind == 'wavpack':
+            h = _decode_blocks(lib, table.data, blocks, stream)
         elif kind == 'alac':
             fl, _, depth, pb, mb, kb, channels, _, _, _, rate = struct.unpack('>IBBBBBBHIII', config[:24])
             cfg = np.array([fl, depth, pb, mb, kb, channels, rate], np.int32)
