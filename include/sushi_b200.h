@@ -39,7 +39,7 @@
 extern "C" {
 #endif
 
-#define SB_ABI_VERSION 10
+#define SB_ABI_VERSION 11
 
 /* status codes */
 #define SB_OK            0
@@ -296,6 +296,19 @@ int sb_alac_decode_frames(const void* buf, int64_t nbytes, const int64_t* offset
  * bitstream that reads past its sub-block; a 16-bit stereo sample above 2^19; a block CRC that disagrees. */
 int sb_wavpack_decode_blocks(const void* buf, int64_t nbytes, const int64_t* table, int64_t n, int32_t channels,
                              int32_t rate, sb_pcm** out);
+
+/* TTA, True Audio (ABI version 11): FFmpeg's `tta` decoder output for format-1 streams of 16 or 24 bits, 24-bit
+ * samples by the top 16 bits of FFmpeg's S32 sample, channels in FFmpeg's order.  `buf` holds the stream's frames back
+ * to back (`nbytes` bytes): frame f starts at offsets[f] (increasing) and ends where frame f + 1 starts, the last at
+ * nbytes; each ends with the CRC-32 of its bitstream.  file_offsets[f] is the byte offset in the file of the frame
+ * (.tta) or of the Matroska block holding it: every error names it with the frame index.  config[0..4] is channels (1
+ * to 8), bits (16 or 24), rate (1 to 2^23 - 1), the frame length (256 * rate / 245) and the last frame's length (0 when
+ * it is a whole frame); every other frame holds a whole frame.  One GPU thread decodes each frame.  It fails on: a
+ * unary run or a code that reads past the frame's bitstream; a Rice parameter above 25; a frame other than the last
+ * that reaches the last frame's length with only its CRC left (FFmpeg's decoder cuts such a frame short); bytes left
+ * between the last sample and the CRC; a CRC that disagrees. */
+int sb_tta_decode_frames(const void* buf, int64_t nbytes, const int64_t* offsets, const int64_t* file_offsets, int64_t n,
+                         const int32_t* config, sb_pcm** out);
 
 /* ---- MPEG transport streams (ABI version 7) ----------------------------------
  *

@@ -14,7 +14,7 @@ LIB_PATH = os.path.join(_HERE, 'libsushi_b200.so')
 
 SB_OK = 0
 SB_U8, SB_F32 = 0, 1
-ABI_VERSION = 10
+ABI_VERSION = 11
 SB_TS_PCM_BLURAY, SB_TS_TRUEHD = 0, 1
 
 c_i64 = ctypes.c_int64
@@ -78,6 +78,7 @@ PROTOTYPES = {
     'sb_alac_decode_frames': (ctypes.c_int, [c_vp, c_i64, c_i64p, c_i64p, c_i64, c_i32p, ctypes.POINTER(c_vp)]),
     'sb_wavpack_decode_blocks': (ctypes.c_int, [c_vp, c_i64, c_i64p, c_i64, ctypes.c_int32, ctypes.c_int32,
                                                 ctypes.POINTER(c_vp)]),
+    'sb_tta_decode_frames': (ctypes.c_int, [c_vp, c_i64, c_i64p, c_i64p, c_i64, c_i32p, ctypes.POINTER(c_vp)]),
     'sb_ts_open': (ctypes.c_int, [ctypes.c_int, ctypes.c_int32, ctypes.c_int32, ctypes.POINTER(c_vp)]),
     'sb_ts_feed': (ctypes.c_int, [c_vp, c_vp, c_i64, c_i64]),
     'sb_ts_finish': (ctypes.c_int, [c_vp, c_i32p, ctypes.POINTER(c_vp)]),

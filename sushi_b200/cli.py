@@ -1,11 +1,11 @@
 """The Sushi command line: `python -m sushi_b200 --src a.mkv --dst b.mkv -o out.ass`.
 
 Flags, defaults and checks are the reference's (sushi.py:528-843).  --src and --dst are WAV, FLAC, WavPack (.wv),
-Matroska (.mkv, .mka, .mks, .webm), MP4 / QuickTime (.mp4, .m4a, .m4v, .mov) or transport stream files.  For a WAV file
-the reference starts no subprocess either; a FLAC or WavPack file, a Matroska file's FLAC, ALAC, WavPack or PCM track,
-an MP4 file's ALAC, FLAC
-or PCM track, or a transport stream's (.m2ts, .mts, .m2t, .ts) BD-LPCM or TrueHD stream, is decoded on the GPU, where
-the reference would have ffmpeg convert it to a WAV file (DESIGN.md section 2): no WAV file is ever written.  A Matroska input also gives, as the reference's ffmpeg and
+TTA (.tta), Matroska (.mkv, .mka, .mks, .webm), MP4 / QuickTime (.mp4, .m4a, .m4v, .mov) or transport stream files.
+For a WAV file the reference starts no subprocess either; a FLAC, WavPack or TTA file, a Matroska file's FLAC, ALAC,
+WavPack, TTA or PCM track, an MP4 file's ALAC, FLAC or PCM track, or a transport stream's (.m2ts, .mts, .m2t, .ts)
+BD-LPCM or TrueHD stream, is decoded on the GPU, where the reference would have ffmpeg convert it to a WAV file
+(DESIGN.md section 2): no WAV file is ever written.  A Matroska input also gives, as the reference's ffmpeg and
 mkvextract calls do, the script, the chapters and the video timestamps (sushi_b200.matroska); those are written to
 the reference's temporary paths and removed at the end unless --no-cleanup is given.  Every check runs before the GPU
 is touched; the run itself is pipeline.shift_script.
@@ -18,7 +18,7 @@ import sys
 import time
 
 from . import __version__
-from . import matroska, mp4, mpegts, wavpack
+from . import matroska, mp4, mpegts, tta, wavpack
 from .common import SushiError
 from .pipeline import shift_script
 from .script import format_srt_time
@@ -110,9 +110,9 @@ def create_arg_parser():
                         help='Timecodes file to use instead of making one from the source (when possible)')
 
     parser.add_argument('--src', required=True, dest='source', metavar='<filename>',
-                        help='Source audio or video (WAV, FLAC, WavPack, TrueHD, Matroska, MP4 or MPEG-TS)')
+                        help='Source audio or video (WAV, FLAC, WavPack, TTA, TrueHD, Matroska, MP4 or MPEG-TS)')
     parser.add_argument('--dst', required=True, dest='destination', metavar='<filename>',
-                        help='Destination audio or video (WAV, FLAC, WavPack, TrueHD, Matroska, MP4 or MPEG-TS)')
+                        help='Destination audio or video (WAV, FLAC, WavPack, TTA, TrueHD, Matroska, MP4 or MPEG-TS)')
     parser.add_argument('-o', '--output', default=None, dest='output_script', metavar='<filename>',
                         help='Output script')
 
@@ -123,12 +123,15 @@ def create_arg_parser():
 
 
 def _open_input(path):
-    """None for a WAV, FLAC, raw TrueHD (.thd) or raw WavPack (.wv) input; the opened MatroskaFile for a Matroska one, the opened
+    """None for a WAV, FLAC, raw TrueHD (.thd), raw WavPack (.wv) or raw TTA (.tta) input; the opened MatroskaFile for a Matroska one, the opened
     TransportStream for a transport stream (.m2ts, .mts, .m2t, .ts).  Anything else, or a Matroska or transport stream
     name that does not open as one, is refused where the reference would have ffmpeg demux it."""
     ext = get_extension(path)
     if ext in wavpack.WV_EXTENSIONS:
         wavpack.WavPackFile(path)                  # its refusals, before the GPU is touched
+        return None
+    if ext in tta.TTA_EXTENSIONS:
+        tta.TTAFile(path)                          # its refusals, before the GPU is touched
         return None
     if ext in ('.wav', '.flac', '.thd'):
         return None

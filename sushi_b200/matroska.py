@@ -24,7 +24,7 @@ import zlib
 
 import numpy as np
 
-from . import wavpack
+from . import tta, wavpack
 from .common import SushiError, py2_round, select_stream
 
 EBML_MAGIC = b'\x1a\x45\xdf\xa3'
@@ -36,6 +36,7 @@ ID_SEEKHEAD, ID_INFO, ID_TRACKS, ID_CHAPTERS = 0x114D9B74, 0x1549A966, 0x1654AE6
 ID_CLUSTER, ID_CUES, ID_TAGS, ID_ATTACHMENTS = 0x1F43B675, 0x1C53BB6B, 0x1254C367, 0x1941A469
 ID_VOID, ID_CRC32 = 0xEC, 0xBF
 ID_TIMESTAMP_SCALE = 0x2AD7B1
+ID_DURATION = 0x4489
 ID_TRACK_ENTRY, ID_TRACK_NUMBER, ID_TRACK_TYPE, ID_CODEC_ID, ID_CODEC_PRIVATE = 0xAE, 0xD7, 0x83, 0x86, 0x63A2
 ID_FLAG_DEFAULT, ID_NAME, ID_LANGUAGE, ID_DEFAULT_DURATION = 0x88, 0x536E, 0x22B59C, 0x23E383
 ID_AUDIO, ID_SAMPLING_FREQUENCY, ID_CHANNELS, ID_BIT_DEPTH = 0xE1, 0xB5, 0x9F, 0x6264
@@ -230,6 +231,7 @@ class MatroskaFile(object):
         self._own = fileobj is None
         self._src = _Source(open(path, 'rb', buffering=0) if fileobj is None else fileobj)
         self.timestamp_scale = 1000000
+        self.duration = None                # the Segment's Duration in TimestampScale units (None without one)
         self.tracks, self.chapter_starts = [], []
         self._clusters = []                 # (offset, declared end or None)
         self._tables = {}                   # (stream id, payloads read) -> FrameTable
@@ -343,6 +345,8 @@ class MatroskaFile(object):
                     for cid, b, _ in children(body, where=pos + hl):
                         if cid == ID_TIMESTAMP_SCALE:
                             self.timestamp_scale = _uint(b)
+                        elif cid == ID_DURATION:
+                            self.duration = _float(b)
                 elif eid == ID_TRACKS:
                     self._read_tracks(body, pos + hl)
                     have_tracks = True
@@ -685,9 +689,9 @@ class MatroskaFile(object):
 
 
 def audio_codec(track):
-    """'flac', 'truehd', 'alac', 'wavpack' or 'pcm' for an audio track the GPU loader decodes (FLAC, Dolby TrueHD, ALAC,
-    whose CodecPrivate is the ALACSpecificConfig, WavPack stream versions 0x402-0x410, little-endian integer PCM of 16
-    or 24 bits);
+    """'flac', 'truehd', 'alac', 'wavpack', 'tta' or 'pcm' for an audio track the GPU loader decodes (FLAC, Dolby
+    TrueHD, ALAC, whose CodecPrivate is the ALACSpecificConfig, WavPack stream versions 0x402-0x410, TTA of 16 or 24
+    bits and 1 to 8 channels, little-endian integer PCM of 16 or 24 bits);
     SushiError naming the track and its codec for anything else."""
     if track.refusal:
         raise SushiError(track.refusal)
@@ -702,8 +706,11 @@ def audio_codec(track):
     if track.codec_id == 'A_WAVPACK4':
         wavpack.check_version(track.codec_private, track.id)
         return 'wavpack'
+    if track.codec_id == 'A_TTA1':
+        tta.check_track(track)
+        return 'tta'
     what = track.codec_id + (' at {0} bits'.format(track.bit_depth) if track.codec_id.startswith('A_PCM') else '')
-    raise SushiError('Audio track {0} is {1}, which cannot be decoded here (FLAC, TrueHD, ALAC, WavPack and 16- or '
+    raise SushiError('Audio track {0} is {1}, which cannot be decoded here (FLAC, TrueHD, ALAC, WavPack, TTA and 16- or '
                      '24-bit little-endian PCM can): convert it to FLAC or WAV first'.format(track.id, what))
 
 

@@ -24,7 +24,7 @@ from time import time
 
 import numpy as np
 
-from . import _native, matroska, mp4, mpegts, truehd, wavpack
+from . import _native, matroska, mp4, mpegts, truehd, tta, wavpack
 from ._nvtx import nvtx_range
 from .common import SushiError, clip, py2_round
 
@@ -215,7 +215,7 @@ class FlacFile(object):
             raise SushiError('FLAC with {0} bits per sample is not supported (16 or 24)'.format(self.bits_per_sample))
 
 
-_CODEC_NAMES = {'flac': 'FLAC', 'alac': 'ALAC', 'truehd': 'TrueHD', 'pcm_bluray': 'BD-LPCM', 'wavpack': 'WavPack'}
+_CODEC_NAMES = {'flac': 'FLAC', 'alac': 'ALAC', 'truehd': 'TrueHD', 'pcm_bluray': 'BD-LPCM', 'wavpack': 'WavPack', 'tta': 'TTA'}
 
 
 def _refuse_host(path, codec, loader):
@@ -383,6 +383,8 @@ class WavStream(StreamGeometry):
             name, load = 'TrueHD', self._load_truehd
         elif wavpack.is_wavpack(path):
             name, load = 'WavPack', self._load_wavpack
+        elif tta.is_tta(path):
+            name, load = 'TTA', self._load_tta
         elif is_flac(path):
             name, load = 'FLAC', self._load_flac
         else:
@@ -443,6 +445,18 @@ class WavStream(StreamGeometry):
         self._load_decoded(_decode_blocks(_native.lib(device), f.data, f.table, f.stream), sample_rate, sample_type,
                            device)
 
+    def _load_tta(self, path, sample_rate, sample_type, device, loader, track):
+        """A raw TTA (.tta) file: its header and seek table read on the host (tta.TTAFile, which refuses what cannot be
+        decoded and damage they show), every frame decoded on the GPU (sb_tta_decode_frames)."""
+        f = tta.TTAFile(path)
+        _refuse_host(path, 'TTA', loader)
+        # the file's bytes as read, up to the end of the audio: frames at their file offsets, no copy
+        buf = np.frombuffer(f.data, dtype=np.uint8)
+        h = _decode(_native.lib(device), 'sb_tta_decode_frames', buf.ctypes.data_as(ctypes.c_void_p), f.end,
+                    f.where.ctypes.data_as(_native.c_i64p), f.where.ctypes.data_as(_native.c_i64p), len(f.where),
+                    f.config.ctypes.data_as(_native.c_i32p))
+        self._load_decoded(h, sample_rate, sample_type, device)
+
     def _load_ts(self, path, sample_rate, sample_type, device, loader, track):
         """A transport stream's BD-LPCM or TrueHD stream (sb_ts_*).  The file is read in chunks of mpegts.CHUNK_BYTES
         into two page-locked buffers, one after the other, so that the GPU scans one chunk while the next is read."""
@@ -488,6 +502,9 @@ class WavStream(StreamGeometry):
             pcm = (t.channels, int(t.sampling_frequency), t.bit_depth // 8, False) if kind == 'pcm' else None
             # WavPack: the stream version, and the channel count a multi-block frame must code
             config = (t.codec_private, t.channels) if kind == 'wavpack' else t.codec_private
+            if kind == 'tta':
+                # the decoder config FFmpeg builds from the track and the Segment's Duration
+                config = tta.matroska_config(t, mkv.timestamp_scale, mkv.duration)
             self._load_track(mkv.path, t.id, kind, config, pcm, read_frames, sample_rate, sample_type, device,
                              loader)
         finally:
@@ -511,10 +528,10 @@ class WavStream(StreamGeometry):
 
     def _load_track(self, path, track_id, kind, config, pcm, read_frames, sample_rate, sample_type, device, loader):
         """A container's audio track loads exactly as the plain PCM WAV of the samples FFmpeg's decoder returns, frames
-        concatenated in container order (timestamp gaps are not filled).  `kind` is 'flac', 'alac', 'truehd', 'wavpack'
-        or 'pcm'; `config` the codec's configuration (FLAC metadata blocks, the ALACSpecificConfig, WavPack's
-        (CodecPrivate, channel count)); `pcm` (channels, rate, sample width, big-endian) for PCM.  read_frames() reads
-        the track's FrameTable, only once every refusal has passed.  FLAC, ALAC, WavPack and TrueHD frames are
+        concatenated in container order (timestamp gaps are not filled).  `kind` is 'flac', 'alac', 'truehd', 'wavpack',
+        'tta' or 'pcm'; `config` the codec's configuration (FLAC metadata blocks, the ALACSpecificConfig, WavPack's
+        (CodecPrivate, channel count), TTA's decoder config); `pcm` (channels, rate, sample width, big-endian) for PCM.  read_frames() reads
+        the track's FrameTable, only once every refusal has passed.  FLAC, ALAC, WavPack, TTA and TrueHD frames are
         decoded on the GPU where the table puts them, errors naming the file offset of a frame's block; PCM goes through sb_load_pcm (little-endian), sb_pcm_from_be (big-endian) or, for
         loader='host', the host loader."""
         name = '{0} track {1}'.format(path, track_id)
@@ -550,6 +567,9 @@ class WavStream(StreamGeometry):
                                info.bits_per_sample, info.framerate)
         elif kind == 'wavpack':
             h = _decode_blocks(lib, table.data, blocks, stream)
+        elif kind == 'tta':
+            h = _decode_frames(lib, 'sb_tta_decode_frames', table.data, table.offset, table.block,
+                               config.ctypes.data_as(_native.c_i32p))
         elif kind == 'alac':
             fl, _, depth, pb, mb, kb, channels, _, _, _, rate = struct.unpack('>IBBBBBBHIII', config[:24])
             cfg = np.array([fl, depth, pb, mb, kb, channels, rate], np.int32)
