@@ -14,6 +14,9 @@
 // are 64-bit.
 #pragma once
 #include <stdint.h>
+#include <vector>
+
+#include "sb_frames.h"
 
 #if defined(__CUDACC__)
 #define SBA_HD __host__ __device__ __forceinline__
@@ -332,6 +335,53 @@ SBA_HD int decode_frame(const uint8_t* buf, int64_t offset, int64_t limit, const
     if (ch == 0) return kNoElement;
     if (ch != c.channels) return kFewChannels;
     return kOk;
+}
+
+// ---- host side: what sb_alac_decode_frames does around the kernels; the CPU build of the tests runs the same ----
+
+// config[0..7) (frameLength, bitDepth, pb, mb, kb, channels, rate) into *c.  Returns false with a message.
+inline bool parse_config(const int32_t* config, Config* c, char* msg, size_t msg_len) {
+    c->frame_length = config[0]; c->bit_depth = config[1]; c->pb = config[2]; c->mb = config[3];
+    c->kb = config[4]; c->channels = config[5]; c->rate = config[6];
+    if (c->bit_depth != 16 && c->bit_depth != 20 && c->bit_depth != 24 && c->bit_depth != 32)
+        snprintf(msg, msg_len, "ALAC with %d bits per sample is not supported (16, 20, 24 or 32)", c->bit_depth);
+    else if (c->frame_length < 1 || c->frame_length > kMaxFrameLength)
+        snprintf(msg, msg_len, "ALAC frameLength %d is not supported (1 to %d)", c->frame_length, kMaxFrameLength);
+    else if (c->channels < 1 || c->channels > 8)
+        snprintf(msg, msg_len, "ALAC with %d channels is not supported (1 to 8)", c->channels);
+    else if (c->rate < 1 || c->pb < 0 || c->pb > 255 || c->mb < 0 || c->mb > 255 || c->kb < 0 || c->kb > 255)
+        snprintf(msg, msg_len, "sb_alac_decode_frames: bad stream parameters");
+    else
+        return true;
+    return false;
+}
+
+// Frame f holds bytes [offsets[f], offsets[f + 1]) of the buffer, the last up to nbytes: every frame must start
+// inside the buffer and hold a byte.  `where` names each frame's file offset.  Returns false with a message.
+inline bool check_offsets(const int64_t* offsets, const int64_t* where, int64_t n, int64_t nbytes, char* msg,
+                          size_t msg_len) {
+    for (int64_t f = 0; f < n; ++f) {
+        const int64_t end = f + 1 < n ? offsets[f + 1] : nbytes;
+        if (offsets[f] < 0 || offsets[f] >= nbytes)
+            return sbframes::refuse(msg, msg_len, "ALAC frame", f, where[f], "frame starts outside the buffer");
+        if (end <= offsets[f]) return sbframes::refuse(msg, msg_len, "ALAC frame", f, where[f], "empty frame");
+    }
+    return true;
+}
+
+// The frame table from what k_alac_frames read: sample positions are the prefix sum of the frames' sample counts.
+// Returns false with the message of the first frame whose first element was refused.
+inline bool frame_table(const Listed* listed, const int64_t* offsets, const int64_t* where, int64_t n, int64_t nbytes,
+                        std::vector<FrameDesc>& frames, int64_t* samples, char* msg, size_t msg_len) {
+    frames.resize((size_t)n);
+    int64_t sample = 0;
+    for (int64_t f = 0; f < n; ++f) {
+        if (listed[f].code != kOk) return sbframes::refuse(msg, msg_len, "ALAC frame", f, where[f], error_text(listed[f].code));
+        frames[(size_t)f] = FrameDesc{offsets[f], f + 1 < n ? offsets[f + 1] : nbytes, sample};
+        sample += listed[f].samples;
+    }
+    *samples = sample;
+    return true;
 }
 
 }  // namespace sbalac

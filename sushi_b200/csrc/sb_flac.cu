@@ -10,7 +10,7 @@
 //                   previous one ends) and checks the frame's CRC-16 and end; k_flac_decorrelate: one CTA per frame
 //                   undoes the stereo decorrelation and writes int16 (24-bit: the top 16 bits) into an sb_pcm
 // The per-frame arithmetic is in sb_flac.cuh, shared with the CPU emulation of the tests.
-#include "sb_internal.h"
+#include "sb_decode.h"
 #include "sb_flac.cuh"
 #include <algorithm>
 #include <vector>
@@ -87,40 +87,29 @@ namespace {
 
 // A FLAC input on the device and its frame table while it is decoded; the upload is freed with it
 struct FlacInput {
+    Blocks blocks;
     uint8_t* d_file = nullptr;
     int64_t nbytes = 0;
     int channels = 0, bits = 0, framerate = 0;
     std::vector<FrameDesc> frames;
     const int64_t* where = nullptr;    // sb_flac_decode_frames: file offset of each frame's block (messages name it)
     int64_t samples = 0;
-    ~FlacInput() { pool_free(d_file); }
 };
-
-// the input on the device, zero-padded past nbytes & ~3 for k_flac_sync
-int upload(FlacInput& h, const void* file, const char* who) {
-    Ctx& c = ctx();
-    SB_TRY(pool_alloc((void**)&h.d_file, (size_t)h.nbytes + 16));
-    cudaError_t e = cudaMemsetAsync(h.d_file + (h.nbytes & ~(int64_t)3), 0, 16, c.stream);
-    if (e == cudaSuccess) e = cudaMemcpyAsync(h.d_file, file, (size_t)h.nbytes, cudaMemcpyHostToDevice, c.stream);
-    if (e != cudaSuccess) SB_FAIL(SB_ECUDA, "%s: %s", who, cudaGetErrorString(e));
-    return SB_OK;
-}
 
 // k_flac_decode, the frame checks, k_flac_decorrelate: the int16 PCM of every frame of h.frames
 int decode(const FlacInput& h, sb_pcm** out, const char* who) {
     Ctx& c = ctx();
     const int64_t nf = (int64_t)h.frames.size();
     const int ch = h.channels;
+    Blocks blocks;
     FrameDesc* d_frames = nullptr;
     int32_t* d_planar = nullptr;
     int16_t* d_pcm = nullptr;
     sbflac::FrameStatus* d_status = nullptr;
-    int rc = pool_alloc((void**)&d_frames, sizeof(FrameDesc) * nf + 16);
-    if (rc == SB_OK) rc = pool_alloc((void**)&d_planar, sizeof(int32_t) * (size_t)h.samples * ch + 16);
-    if (rc == SB_OK) rc = pool_alloc((void**)&d_pcm, sizeof(int16_t) * (size_t)h.samples * ch + 16);
-    if (rc == SB_OK) rc = pool_alloc((void**)&d_status, sizeof(sbflac::FrameStatus) * nf + 16);
-    auto release = [&]() { pool_free(d_frames); pool_free(d_planar); pool_free(d_status); };
-    if (rc != SB_OK) { release(); pool_free(d_pcm); return rc; }
+    SB_TRY(blocks.alloc(&d_frames, (size_t)nf));
+    SB_TRY(blocks.alloc(&d_planar, (size_t)h.samples * ch));
+    SB_TRY(blocks.alloc(&d_pcm, (size_t)h.samples * ch));
+    SB_TRY(blocks.alloc(&d_status, (size_t)nf));
     std::vector<sbflac::FrameStatus> status((size_t)nf);
     cudaError_t e = cudaMemcpyAsync(d_frames, h.frames.data(), sizeof(FrameDesc) * nf, cudaMemcpyHostToDevice, c.stream);
     if (e == cudaSuccess && nf > 0) {
@@ -129,21 +118,15 @@ int decode(const FlacInput& h, sb_pcm** out, const char* who) {
                                                                        d_planar, d_status);
         e = cudaGetLastError();
     }
-    if (e == cudaSuccess) e = cudaMemcpyAsync(status.data(), d_status, sizeof(sbflac::FrameStatus) * nf,
-                                              cudaMemcpyDeviceToHost, c.stream);
-    if (e == cudaSuccess) e = cudaStreamSynchronize(c.stream);
-    if (e != cudaSuccess) { release(); pool_free(d_pcm); SB_FAIL(SB_ECUDA, "%s: %s", who, cudaGetErrorString(e)); }
+    SB_TRY(collect(e, status.data(), d_status, nf, who));
     // every frame must decode, pass its CRC-16 and end exactly where the next frame (or the file) does
     char msg[256];
     auto bytes_at = [&](int64_t off, uint8_t* buf) {
         if (off < h.nbytes) cudaMemcpy(buf, h.d_file + off, (size_t)std::min<int64_t>(16, h.nbytes - off), cudaMemcpyDeviceToHost);
     };
     if (!sbflac::check_frames(h.frames, status.data(), h.nbytes, ch, h.bits, h.framerate, bytes_at, msg, sizeof(msg),
-                              h.where)) {
-        release();
-        pool_free(d_pcm);
+                              h.where))
         SB_FAIL(SB_EINVAL, "%s", msg);
-    }
     if (nf > 0) {
         ProfScope ps("flac_decorrelate");
         k_flac_decorrelate<<<(unsigned)std::max<int64_t>(1, std::min<int64_t>(nf, (int64_t)c.sm_count * 64)), 256, 0,
@@ -151,9 +134,8 @@ int decode(const FlacInput& h, sb_pcm** out, const char* who) {
         e = cudaGetLastError();
     }
     if (e == cudaSuccess) e = cudaStreamSynchronize(c.stream);
-    release();
-    if (e != cudaSuccess) { pool_free(d_pcm); SB_FAIL(SB_ECUDA, "%s: %s", who, cudaGetErrorString(e)); }
-    return pcm_handle(d_pcm, h.samples, ch, h.framerate, out);
+    SB_TRY(cuda_result(e, who));
+    return pcm_handle(blocks.take(d_pcm), h.samples, ch, h.framerate, out);
 }
 
 }  // namespace
@@ -162,62 +144,41 @@ extern "C" {
 
 int sb_flac_decode_file(const void* file, int64_t nbytes, int64_t first_frame_offset, int channels, int bits,
                         int framerate, sb_pcm** out) {
+    const char* who = "sb_flac_decode_file";
     Ctx& c = ctx();
-    if (!c.inited) SB_FAIL(SB_ESTATE, "sb_flac_decode_file: library not initialised (call sb_init)");
-    if (!file || !out) SB_FAIL(SB_EINVAL, "sb_flac_decode_file: NULL argument");
+    SB_TRY(entry_check(who, file && out));
     if (bits != 16 && bits != 24) SB_FAIL(SB_EINVAL, "FLAC with %d bits per sample is not supported (16 or 24)", bits);
     if (channels < 1 || channels > 8 || framerate < 1 || nbytes < 1 || first_frame_offset < 0 || first_frame_offset > nbytes)
         SB_FAIL(SB_EINVAL, "sb_flac_decode_file: bad stream parameters");
     FlacInput h;
     h.nbytes = nbytes; h.channels = channels; h.bits = bits; h.framerate = framerate;
     const uint8_t* host = static_cast<const uint8_t*>(file);
-    SB_TRY(upload(h, file, "sb_flac_decode_file"));
+    SB_TRY(upload_padded(h.blocks, &h.d_file, file, nbytes, who));
 
     // candidates: a frame has at least 9 bytes; real files hold one frame per few kB and false syncs are rarer still
-    int64_t cap = nbytes / 256 + 4096;
     std::vector<Candidate> cand;
-    for (int pass = 0; pass < 2; ++pass) {
-        Candidate* d_cand = nullptr;
-        unsigned long long* d_count = nullptr;
-        if (pool_alloc((void**)&d_cand, sizeof(Candidate) * cap) != SB_OK) return SB_ENOMEM;
-        if (pool_alloc((void**)&d_count, sizeof(unsigned long long)) != SB_OK) { pool_free(d_cand); return SB_ENOMEM; }
-        unsigned long long count = 0;
-        cudaError_t e = cudaMemsetAsync(d_count, 0, sizeof(unsigned long long), c.stream);
-        if (e == cudaSuccess) {
-            ProfScope ps("flac_sync");
-            const int64_t words = (nbytes + 3) / 4;
-            const int grid = (int)std::min<int64_t>((words + 255) / 256, (int64_t)c.sm_count * 16);
-            k_flac_sync<<<std::max(grid, 1), 256, 0, c.stream>>>(h.d_file, first_frame_offset, nbytes, channels, bits,
-                                                                 framerate, d_cand, d_count, cap);
-            e = cudaGetLastError();
-        }
-        if (e == cudaSuccess) e = cudaMemcpyAsync(&count, d_count, sizeof(count), cudaMemcpyDeviceToHost, c.stream);
-        if (e == cudaSuccess) e = cudaStreamSynchronize(c.stream);
-        if (e == cudaSuccess && (int64_t)count <= cap) {
-            cand.resize(count);
-            e = cudaMemcpyAsync(cand.data(), d_cand, sizeof(Candidate) * count, cudaMemcpyDeviceToHost, c.stream);
-            if (e == cudaSuccess) e = cudaStreamSynchronize(c.stream);
-        }
-        pool_free(d_cand); pool_free(d_count);
-        if (e != cudaSuccess) SB_FAIL(SB_ECUDA, "sb_flac_decode_file: %s", cudaGetErrorString(e));
-        if ((int64_t)count <= cap) break;
-        cap = (int64_t)count;                                              // rescan with room for every candidate
-    }
+    SB_TRY(scan_candidates(nbytes / 256 + 4096, "flac_sync", who, [&](Candidate* d_cand, unsigned long long* d_count, int64_t cap) {
+        const int64_t words = (nbytes + 3) / 4;
+        const int grid = (int)std::min<int64_t>((words + 255) / 256, (int64_t)c.sm_count * 16);
+        k_flac_sync<<<std::max(grid, 1), 256, 0, c.stream>>>(h.d_file, first_frame_offset, nbytes, channels, bits,
+                                                             framerate, d_cand, d_count, cap);
+    }, cand));
     char msg[256];
     if (!sbflac::chain(cand, first_frame_offset, nbytes, channels, bits, framerate, host + first_frame_offset, h.frames,
                        &h.samples, msg, sizeof(msg)))
         SB_FAIL(SB_EINVAL, "%s", msg);
-    return decode(h, out, "sb_flac_decode_file");
+    return decode(h, out, who);
 }
 
 int sb_flac_decode_frames(const void* buf, int64_t nbytes, const int64_t* offsets, const int64_t* file_offsets, int64_t n,
                           int channels, int bits, int framerate, sb_pcm** out) {
+    const char* who = "sb_flac_decode_frames";
     Ctx& c = ctx();
-    if (!c.inited) SB_FAIL(SB_ESTATE, "sb_flac_decode_frames: library not initialised (call sb_init)");
-    if (!buf || !offsets || !file_offsets || !out) SB_FAIL(SB_EINVAL, "sb_flac_decode_frames: NULL argument");
+    SB_TRY(entry_check(who, buf && offsets && file_offsets && out));
     if (bits != 16 && bits != 24) SB_FAIL(SB_EINVAL, "FLAC with %d bits per sample is not supported (16 or 24)", bits);
     if (channels < 1 || channels > 8 || framerate < 1 || nbytes < 1 || n < 0)
         SB_FAIL(SB_EINVAL, "sb_flac_decode_frames: bad stream parameters");
+    // a frame ends where the next one starts: here the frame named is the one that starts at or before its predecessor
     for (int64_t f = 0; f < n; ++f)
         if (offsets[f] < 0 || offsets[f] >= nbytes || (f > 0 && offsets[f] <= offsets[f - 1]))
             SB_FAIL(SB_EINVAL, "FLAC frame %lld at byte offset %lld: %s", (long long)f, (long long)file_offsets[f],
@@ -225,28 +186,27 @@ int sb_flac_decode_frames(const void* buf, int64_t nbytes, const int64_t* offset
     FlacInput h;
     h.nbytes = nbytes; h.channels = channels; h.bits = bits; h.framerate = framerate;
     h.where = file_offsets;
-    SB_TRY(upload(h, buf, "sb_flac_decode_frames"));
-    int64_t* d_offsets = nullptr;
-    sbflac::ListedFrame* d_listed = nullptr;
-    if (pool_alloc((void**)&d_offsets, sizeof(int64_t) * n + 16) != SB_OK) return SB_ENOMEM;
-    if (pool_alloc((void**)&d_listed, sizeof(sbflac::ListedFrame) * n + 16) != SB_OK) { pool_free(d_offsets); return SB_ENOMEM; }
+    SB_TRY(upload_padded(h.blocks, &h.d_file, buf, nbytes, who));
     std::vector<sbflac::ListedFrame> listed((size_t)n);
-    cudaError_t e = cudaMemcpyAsync(d_offsets, offsets, sizeof(int64_t) * n, cudaMemcpyHostToDevice, c.stream);
-    if (e == cudaSuccess && n > 0) {
-        ProfScope ps("flac_frames");
-        k_flac_frames<<<(unsigned)((n + 255) / 256), 256, 0, c.stream>>>(h.d_file, nbytes, d_offsets, n, channels, bits,
-                                                                         framerate, d_listed);
-        e = cudaGetLastError();
+    {
+        Blocks blocks;
+        int64_t* d_offsets = nullptr;
+        sbflac::ListedFrame* d_listed = nullptr;
+        SB_TRY(blocks.alloc(&d_offsets, (size_t)n));
+        SB_TRY(blocks.alloc(&d_listed, (size_t)n));
+        cudaError_t e = cudaMemcpyAsync(d_offsets, offsets, sizeof(int64_t) * n, cudaMemcpyHostToDevice, c.stream);
+        if (e == cudaSuccess && n > 0) {
+            ProfScope ps("flac_frames");
+            k_flac_frames<<<(unsigned)((n + 255) / 256), 256, 0, c.stream>>>(h.d_file, nbytes, d_offsets, n, channels,
+                                                                             bits, framerate, d_listed);
+            e = cudaGetLastError();
+        }
+        SB_TRY(collect(e, listed.data(), d_listed, n, who));
     }
-    if (e == cudaSuccess) e = cudaMemcpyAsync(listed.data(), d_listed, sizeof(sbflac::ListedFrame) * n,
-                                              cudaMemcpyDeviceToHost, c.stream);
-    if (e == cudaSuccess) e = cudaStreamSynchronize(c.stream);
-    pool_free(d_offsets); pool_free(d_listed);
-    if (e != cudaSuccess) SB_FAIL(SB_ECUDA, "sb_flac_decode_frames: %s", cudaGetErrorString(e));
     char msg[256];
     if (!sbflac::list_frames(listed.data(), offsets, file_offsets, n, nbytes, h.frames, &h.samples, msg, sizeof(msg)))
         SB_FAIL(SB_EINVAL, "%s", msg);
-    return decode(h, out, "sb_flac_decode_frames");
+    return decode(h, out, who);
 }
 
 }  // extern "C"

@@ -7,7 +7,7 @@
 //                     which decodes its AUs in turn into int16 at AU index x samples per AU and returns its lossless
 //                     check; the host joins the checks of neighbouring segments
 // The per-AU arithmetic is in sb_truehd.cuh, shared with the CPU emulation of the tests.
-#include "sb_internal.h"
+#include "sb_decode.h"
 #include "sb_truehd.cuh"
 #include <algorithm>
 #include <functional>
@@ -55,7 +55,7 @@ k_truehd_decode(const uint8_t* __restrict__ buf, int64_t nbytes, const int64_t* 
 namespace sb {
 
 // The body of sb_truehd_decode on a stream already on the device: `host` and `d_buf` hold the same `nbytes` bytes (d_buf
-// zero-padded to 16 bytes past nbytes & ~3 for k_truehd_sync); blocks start at offsets[0..n) (d_blocks: the same on
+// followed by the zero bytes of sb_decode.h's contract, for k_truehd_sync); blocks start at offsets[0..n) (d_blocks: the same on
 // the device); where(off) is the file offset messages give for stream byte `off`.  The caller keeps d_buf and d_blocks.
 int truehd_index_device(const uint8_t* host, const uint8_t* d_buf, int64_t nbytes, const int64_t* offsets,
                         const int64_t* d_blocks, int64_t n, const std::function<int64_t(int64_t)>& where, sb_pcm** out) {
@@ -66,64 +66,36 @@ int truehd_index_device(const uint8_t* host, const uint8_t* d_buf, int64_t nbyte
         snprintf(msg, sizeof(msg), fmsg, (long long)where(offsets[0]));
         SB_FAIL(SB_EINVAL, "%s", msg);
     }
-    cudaError_t e = cudaSuccess;
+    const char* who = "sb_truehd_decode";       // a transport stream's payload comes through sb_ts_finish: same name
 
     // candidates: a major sync opens every 1 to 128 AUs of at least a few dozen bytes
-    int64_t cap = nbytes / 512 + 4096;
     std::vector<sbthd::Candidate> cand;
-    for (int pass = 0; pass < 2; ++pass) {
-        sbthd::Candidate* d_cand = nullptr;
-        unsigned long long* d_count = nullptr;
-        if (pool_alloc((void**)&d_cand, sizeof(sbthd::Candidate) * cap) != SB_OK) return SB_ENOMEM;
-        if (pool_alloc((void**)&d_count, sizeof(unsigned long long)) != SB_OK) { pool_free(d_cand); return SB_ENOMEM; }
-        unsigned long long count = 0;
-        e = cudaMemsetAsync(d_count, 0, sizeof(unsigned long long), c.stream);
-        if (e == cudaSuccess) {
-            ProfScope ps("truehd_sync");
-            const int64_t words = (nbytes + 3) / 4;
-            const int grid = (int)std::min<int64_t>((words + 255) / 256, (int64_t)c.sm_count * 16);
-            k_truehd_sync<<<std::max(grid, 1), 256, 0, c.stream>>>(d_buf, nbytes, f, d_cand, d_count, cap);
-            e = cudaGetLastError();
-        }
-        if (e == cudaSuccess) e = cudaMemcpyAsync(&count, d_count, sizeof(count), cudaMemcpyDeviceToHost, c.stream);
-        if (e == cudaSuccess) e = cudaStreamSynchronize(c.stream);
-        if (e == cudaSuccess && (int64_t)count <= cap) {
-            cand.resize(count);
-            e = cudaMemcpyAsync(cand.data(), d_cand, sizeof(sbthd::Candidate) * count, cudaMemcpyDeviceToHost, c.stream);
-            if (e == cudaSuccess) e = cudaStreamSynchronize(c.stream);
-        }
-        pool_free(d_cand); pool_free(d_count);
-        if (e != cudaSuccess) SB_FAIL(SB_ECUDA, "sb_truehd_decode: %s", cudaGetErrorString(e));
-        if ((int64_t)count <= cap) break;
-        cap = (int64_t)count;                                              // rescan with room for every candidate
-    }
+    SB_TRY(scan_candidates(nbytes / 512 + 4096, "truehd_sync", who, [&](sbthd::Candidate* d_cand, unsigned long long* d_count, int64_t cap) {
+        const int64_t words = (nbytes + 3) / 4;
+        const int grid = (int)std::min<int64_t>((words + 255) / 256, (int64_t)c.sm_count * 16);
+        k_truehd_sync<<<std::max(grid, 1), 256, 0, c.stream>>>(d_buf, nbytes, f, d_cand, d_count, cap);
+    }, cand));
     std::sort(cand.begin(), cand.end(), [](const sbthd::Candidate& a, const sbthd::Candidate& b) { return a.offset < b.offset; });
     std::vector<sbthd::Segment> segs;
     int64_t n_au = 0;
     if (!sbthd::chain(host, nbytes, offsets, n, cand, where, segs, &n_au, msg, sizeof(msg))) SB_FAIL(SB_EINVAL, "%s", msg);
     const int64_t ns = (int64_t)segs.size();
+    Blocks blocks;
     sbthd::Segment* d_segs = nullptr;
     sbthd::SegStatus* d_status = nullptr;
     int16_t* d_pcm = nullptr;
-    auto fail = [&](int code) { pool_free(d_pcm); return code; };
     std::vector<sbthd::SegStatus> status((size_t)ns);
-    int rc = pool_alloc((void**)&d_pcm, sizeof(int16_t) * (size_t)(n_au * f.spa * f.channels) + 16);
-    if (rc == SB_OK) rc = pool_alloc((void**)&d_segs, sizeof(sbthd::Segment) * ns + 16);
-    if (rc == SB_OK) rc = pool_alloc((void**)&d_status, sizeof(sbthd::SegStatus) * ns + 16);
-    auto release = [&]() { pool_free(d_segs); pool_free(d_status); };
-    if (rc != SB_OK) { release(); return fail(rc); }
-    e = cudaMemcpyAsync(d_segs, segs.data(), sizeof(sbthd::Segment) * ns, cudaMemcpyHostToDevice, c.stream);
+    SB_TRY(blocks.alloc(&d_pcm, (size_t)(n_au * f.spa * f.channels)));
+    SB_TRY(blocks.alloc(&d_segs, (size_t)ns));
+    SB_TRY(blocks.alloc(&d_status, (size_t)ns));
+    cudaError_t e = cudaMemcpyAsync(d_segs, segs.data(), sizeof(sbthd::Segment) * ns, cudaMemcpyHostToDevice, c.stream);
     if (e == cudaSuccess && ns > 0) {
         ProfScope ps("truehd_decode");
         k_truehd_decode<<<(unsigned)((ns + 63) / 64), 64, 0, c.stream>>>(d_buf, nbytes, d_blocks, n, f, d_segs, ns,
                                                                          d_pcm, d_status);
         e = cudaGetLastError();
     }
-    if (e == cudaSuccess) e = cudaMemcpyAsync(status.data(), d_status, sizeof(sbthd::SegStatus) * ns, cudaMemcpyDeviceToHost,
-                                              c.stream);
-    if (e == cudaSuccess) e = cudaStreamSynchronize(c.stream);
-    release();
-    if (e != cudaSuccess) { fail(0); SB_FAIL(SB_ECUDA, "sb_truehd_decode: %s", cudaGetErrorString(e)); }
+    SB_TRY(collect(e, status.data(), d_status, ns, who));
     // messages name the failing AU by the offset of its block: walk the failing segment's AU lengths up to it
     auto where_au = [&](int64_t k, int64_t au) {
         int64_t off = segs[k].offset;
@@ -131,8 +103,8 @@ int truehd_index_device(const uint8_t* host, const uint8_t* d_buf, int64_t nbyte
         return where(off);
     };
     const int64_t frames = sbthd::check_segments(segs, status.data(), f, where_au, msg, sizeof(msg));
-    if (frames < 0) { fail(0); SB_FAIL(SB_EINVAL, "%s", msg); }
-    return pcm_handle(d_pcm, frames, f.channels, f.rate, out);
+    if (frames < 0) SB_FAIL(SB_EINVAL, "%s", msg);
+    return pcm_handle(blocks.take(d_pcm), frames, f.channels, f.rate, out);
 }
 
 }  // namespace sb
@@ -141,9 +113,9 @@ extern "C" {
 
 int sb_truehd_decode(const void* buf, int64_t nbytes, const int64_t* offsets, const int64_t* file_offsets, int64_t n,
                      sb_pcm** out) {
+    const char* who = "sb_truehd_decode";
     Ctx& c = ctx();
-    if (!c.inited) SB_FAIL(SB_ESTATE, "sb_truehd_decode: library not initialised (call sb_init)");
-    if (!buf || !offsets || !file_offsets || !out) SB_FAIL(SB_EINVAL, "sb_truehd_decode: NULL argument");
+    SB_TRY(entry_check(who, buf && offsets && file_offsets && out));
     if (nbytes < 1 || n < 1) SB_FAIL(SB_EINVAL, "sb_truehd_decode: empty stream");
     for (int64_t b = 0; b < n; ++b)
         if (offsets[b] < 0 || offsets[b] >= nbytes || (b > 0 && offsets[b] <= offsets[b - 1]))
@@ -155,20 +127,15 @@ int sb_truehd_decode(const void* buf, int64_t nbytes, const int64_t* offsets, co
         const int64_t b = std::upper_bound(offsets, offsets + n, off) - offsets;
         return b > 0 && file_offsets[b - 1] >= 0 ? file_offsets[b - 1] : off;
     };
+    Blocks blocks;
     uint8_t* d_buf = nullptr;
     int64_t* d_blocks = nullptr;
-    auto release = [&]() { pool_free(d_buf); pool_free(d_blocks); };
-    if (pool_alloc((void**)&d_buf, (size_t)nbytes + 16) != SB_OK || pool_alloc((void**)&d_blocks, sizeof(int64_t) * n + 16) != SB_OK) {
-        release();
-        SB_FAIL(SB_ENOMEM, "sb_truehd_decode: out of device memory");
-    }
-    cudaError_t e = cudaMemsetAsync(d_buf + (nbytes & ~(int64_t)3), 0, 16, c.stream);      // zero tail for k_truehd_sync
-    if (e == cudaSuccess) e = cudaMemcpyAsync(d_buf, buf, (size_t)nbytes, cudaMemcpyHostToDevice, c.stream);
-    if (e == cudaSuccess) e = cudaMemcpyAsync(d_blocks, offsets, sizeof(int64_t) * n, cudaMemcpyHostToDevice, c.stream);
-    if (e != cudaSuccess) { release(); SB_FAIL(SB_ECUDA, "sb_truehd_decode: %s", cudaGetErrorString(e)); }
-    const int rc = truehd_index_device(host, d_buf, nbytes, offsets, d_blocks, n, where, out);
-    release();
-    return rc;
+    int rc = upload_padded(blocks, &d_buf, buf, nbytes, who);
+    if (rc == SB_OK) rc = blocks.alloc(&d_blocks, (size_t)n);
+    if (rc == SB_ENOMEM) SB_FAIL(SB_ENOMEM, "sb_truehd_decode: out of device memory");
+    SB_TRY(rc);
+    SB_TRY(cuda_result(cudaMemcpyAsync(d_blocks, offsets, sizeof(int64_t) * n, cudaMemcpyHostToDevice, c.stream), who));
+    return truehd_index_device(host, d_buf, nbytes, offsets, d_blocks, n, where, out);
 }
 
 }  // extern "C"

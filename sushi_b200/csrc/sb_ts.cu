@@ -15,7 +15,7 @@
 //                  over sample frames into interleaved int16) or k_ts_gather + the TrueHD decoder of sb_truehd.cu, into
 //                  an sb_pcm
 // The per-packet and per-PES rules are in sb_ts.cuh, shared with the CPU emulation of the tests.
-#include "sb_internal.h"
+#include "sb_decode.h"
 #include "sb_ts.cuh"
 #include <algorithm>
 #include <new>
@@ -402,37 +402,34 @@ int scan_i64(int64_t* d_v, int64_t n, int64_t* total) {
 extern "C" {
 
 int sb_ts_finish(sb_ts* t, int32_t* cut, sb_pcm** out) {
+    const char* who = "sb_ts_finish";
     Ctx& c = ctx();
-    if (!c.inited) SB_FAIL(SB_ESTATE, "sb_ts_finish: library not initialised (call sb_init)");
-    if (!t || !cut || !out) SB_FAIL(SB_EINVAL, "sb_ts_finish: NULL argument");
+    SB_TRY(entry_check(who, t && cut && out));
     if (t->finished) SB_FAIL(SB_ESTATE, "sb_ts_finish: the stream is finished");
     t->finished = true;
+    // the demultiplexer's buffers go when this returns, on whichever line: after truehd_index_device, whose `where`
+    // reads t->d_tab when it words a message
+    struct ReleaseDemux { sb_ts* t; ~ReleaseDemux() { t->release_demux(); } } release_demux{t};
     unsigned long long err = kNoError;
-    cudaError_t e = cudaMemcpyAsync(&err, t->d_err, sizeof(err), cudaMemcpyDeviceToHost, c.stream);
-    if (e == cudaSuccess) e = cudaStreamSynchronize(c.stream);
-    if (e != cudaSuccess) { t->release_demux(); SB_FAIL(SB_ECUDA, "sb_ts_finish: %s", cudaGetErrorString(e)); }
+    SB_TRY(collect(cudaSuccess, &err, t->d_err, 1, who));
     const Totals run = *t->h_run;
     auto refuse = [&](unsigned long long code) {
-        t->release_demux();
         const int k = (int)(code & 0xFF);
         SB_FAIL(SB_EINVAL, "%s at byte offset %lld: %s", k <= sbts::kCcGap ? "transport stream packet" : "PES packet",
                 (long long)(code >> 8), sbts::error_text(k));
     };
     if (err != kNoError) return refuse(err);
-    if (run.pes < 1) { t->release_demux(); SB_FAIL(SB_EINVAL, "PID %d carries no PES packet", t->pid); }
+    if (run.pes < 1) SB_FAIL(SB_EINVAL, "PID %d carries no PES packet", t->pid);
     const int64_t n_pes = run.pes;
+    Blocks blocks;
     int64_t* d_off = nullptr;
     int64_t* d_count = nullptr;
     uint32_t* d_misc = nullptr;
-    auto release = [&]() { pool_free(d_off); pool_free(d_count); pool_free(d_misc); t->release_demux(); };
-    if (pool_alloc((void**)&d_off, sizeof(int64_t) * (size_t)n_pes + 16) != SB_OK ||
-        pool_alloc((void**)&d_count, sizeof(int64_t) * (size_t)n_pes + 16) != SB_OK ||
-        pool_alloc((void**)&d_misc, 16) != SB_OK) {
-        release();
+    if (blocks.alloc(&d_off, (size_t)n_pes) != SB_OK || blocks.alloc(&d_count, (size_t)n_pes) != SB_OK ||
+        blocks.alloc(&d_misc, 4) != SB_OK)
         SB_FAIL(SB_ENOMEM, "sb_ts_finish: out of device memory");
-    }
     uint32_t misc[2] = {0, 0};                          // the first BD-LPCM header, the cut flag
-    e = cudaMemsetAsync(d_misc, 0, 16, c.stream);
+    cudaError_t e = cudaMemsetAsync(d_misc, 0, 16, c.stream);
     if (e == cudaSuccess) {
         ProfScope ps("pes_index");
         k_pes_index<<<(unsigned)((n_pes + kThreads - 1) / kThreads), kThreads, 0, c.stream>>>(
@@ -440,23 +437,18 @@ int sb_ts_finish(sb_ts* t, int32_t* cut, sb_pcm** out) {
         e = cudaGetLastError();
     }
     if (e == cudaSuccess) e = cudaMemcpyAsync(&err, t->d_err, sizeof(err), cudaMemcpyDeviceToHost, c.stream);
-    if (e == cudaSuccess) e = cudaMemcpyAsync(misc, d_misc, sizeof(misc), cudaMemcpyDeviceToHost, c.stream);
-    if (e == cudaSuccess) e = cudaStreamSynchronize(c.stream);
-    if (e != cudaSuccess) { release(); SB_FAIL(SB_ECUDA, "sb_ts_finish: %s", cudaGetErrorString(e)); }
-    if (err != kNoError) { pool_free(d_off); pool_free(d_count); pool_free(d_misc); d_off = d_count = nullptr; d_misc = nullptr; return refuse(err); }
+    SB_TRY(collect(e, misc, d_misc, 2, who));
+    if (err != kNoError) return refuse(err);
     // per PES: the first sample frame (LPCM) or the first byte of the TrueHD stream (TrueHD)
     int64_t total = 0;
-    int rc = scan_i64(d_count, n_pes, &total);
-    if (rc != SB_OK) { release(); return rc; }
+    SB_TRY(scan_i64(d_count, n_pes, &total));
     *cut = misc[1] ? 1 : 0;
     if (t->codec == SB_TS_PCM_BLURAY) {
         sbts::Lpcm f;
-        if (sbts::parse_lpcm(misc[0], &f)) { release(); SB_FAIL(SB_EINVAL, "PID %d: no BD-LPCM header", t->pid); }
+        if (sbts::parse_lpcm(misc[0], &f)) SB_FAIL(SB_EINVAL, "PID %d: no BD-LPCM header", t->pid);
         int16_t* d_pcm = nullptr;
-        if (total > 0 && pool_alloc((void**)&d_pcm, sizeof(int16_t) * (size_t)(total * f.channels) + 16) != SB_OK) {
-            release();
+        if (total > 0 && blocks.alloc(&d_pcm, (size_t)(total * f.channels)) != SB_OK)
             SB_FAIL(SB_ENOMEM, "sb_ts_finish: out of device memory for %lld sample frames", (long long)total);
-        }
         if (total > 0) {
             ProfScope ps("bdlpcm_decode");
             const int grid = (int)std::min<int64_t>((total + kThreads - 1) / kThreads, (int64_t)c.sm_count * 16);
@@ -465,40 +457,34 @@ int sb_ts_finish(sb_ts* t, int32_t* cut, sb_pcm** out) {
             e = cudaGetLastError();
         }
         if (e == cudaSuccess) e = cudaStreamSynchronize(c.stream);
-        release();
-        if (e != cudaSuccess) { pool_free(d_pcm); SB_FAIL(SB_ECUDA, "sb_ts_finish: %s", cudaGetErrorString(e)); }
-        return pcm_handle(d_pcm, total, f.channels, f.rate, out);
+        SB_TRY(cuda_result(e, who));
+        return pcm_handle(blocks.take(d_pcm), total, f.channels, f.rate, out);
     }
     // TrueHD: the kept payloads back to back, then the .thd decoder on them as one block
-    if (total < 1) { release(); SB_FAIL(SB_EINVAL, "PID %d carries no TrueHD payload", t->pid); }
+    if (total < 1) SB_FAIL(SB_EINVAL, "PID %d carries no TrueHD payload", t->pid);
     uint8_t* d_thd = nullptr;
     int64_t* d_len = nullptr;
     int64_t* d_block = nullptr;
-    auto release_thd = [&]() { pool_free(d_thd); pool_free(d_len); pool_free(d_block); release(); };
-    if (pool_alloc((void**)&d_thd, (size_t)total + 16) != SB_OK || pool_alloc((void**)&d_len, sizeof(int64_t) * (size_t)n_pes + 16) != SB_OK ||
-        pool_alloc((void**)&d_block, 16) != SB_OK) {
-        release_thd();
+    if (blocks.alloc(&d_thd, (size_t)total) != SB_OK || blocks.alloc(&d_len, (size_t)n_pes) != SB_OK ||
+        blocks.alloc(&d_block, 2) != SB_OK)
         SB_FAIL(SB_ENOMEM, "sb_ts_finish: out of device memory for %lld bytes of TrueHD", (long long)total);
-    }
     std::vector<int64_t> start((size_t)n_pes), off((size_t)n_pes);
     std::vector<uint8_t> host((size_t)total + 1);
     // the lengths again (the scan replaced them by the starts): the difference of consecutive starts
     e = cudaMemcpyAsync(start.data(), d_count, sizeof(int64_t) * (size_t)n_pes, cudaMemcpyDeviceToHost, c.stream);
-    if (e == cudaSuccess) e = cudaMemcpyAsync(off.data(), d_off, sizeof(int64_t) * (size_t)n_pes, cudaMemcpyDeviceToHost, c.stream);
-    if (e == cudaSuccess) e = cudaStreamSynchronize(c.stream);
+    SB_TRY(collect(e, off.data(), d_off, n_pes, who));
     std::vector<int64_t> len((size_t)n_pes);
     for (int64_t s = 0; s < n_pes; ++s) len[(size_t)s] = (s + 1 < n_pes ? start[(size_t)s + 1] : total) - start[(size_t)s];
-    if (e == cudaSuccess) e = cudaMemcpyAsync(d_len, len.data(), sizeof(int64_t) * (size_t)n_pes, cudaMemcpyHostToDevice, c.stream);
-    if (e == cudaSuccess) e = cudaMemsetAsync(d_thd + (total & ~(int64_t)3), 0, 16, c.stream);     // zero tail for k_truehd_sync
+    e = cudaMemcpyAsync(d_len, len.data(), sizeof(int64_t) * (size_t)n_pes, cudaMemcpyHostToDevice, c.stream);
+    // the payload is put together on the device, so its zero tail (sb_decode.h) is written here
+    if (e == cudaSuccess) e = cudaMemsetAsync(d_thd + (total & ~(int64_t)3), 0, 16, c.stream);
     if (e == cudaSuccess) e = cudaMemsetAsync(d_block, 0, 16, c.stream);
     if (e == cudaSuccess) {
         ProfScope ps("ts_compact");
         k_ts_gather<<<(unsigned)n_pes, kThreads, 0, c.stream>>>(t->d_es, d_off, d_len, d_count, d_thd);
         e = cudaGetLastError();
     }
-    if (e == cudaSuccess) e = cudaMemcpyAsync(host.data(), d_thd, (size_t)total, cudaMemcpyDeviceToHost, c.stream);
-    if (e == cudaSuccess) e = cudaStreamSynchronize(c.stream);
-    if (e != cudaSuccess) { release_thd(); SB_FAIL(SB_ECUDA, "sb_ts_finish: %s", cudaGetErrorString(e)); }
+    SB_TRY(collect(e, host.data(), d_thd, total, who));
     // messages name the TS packet holding a TrueHD byte: its PES, its place in the PID's payload, then the packet table
     // (read back only when a message needs it)
     std::vector<PktRec> tab;
@@ -517,9 +503,7 @@ int sb_ts_finish(sb_ts* t, int32_t* cut, sb_pcm** out) {
         return k >= 0 ? tab[(size_t)k].file_off : -1;
     };
     const int64_t zero = 0;
-    rc = truehd_index_device(host.data(), d_thd, total, &zero, d_block, 1, where, out);
-    release_thd();
-    return rc;
+    return truehd_index_device(host.data(), d_thd, total, &zero, d_block, 1, where, out);
 }
 
 int sb_ts_destroy(sb_ts* t) {

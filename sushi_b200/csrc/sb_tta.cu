@@ -7,7 +7,7 @@
 //                  shares one slice-by-4 CRC table there; nothing is kept per frame in global scratch, so every frame
 //                  goes in one launch.
 // The per-frame arithmetic is in sb_tta.cuh, shared with the CPU emulation of the tests.
-#include "sb_internal.h"
+#include "sb_decode.h"
 #include "sb_tta.cuh"
 #include <algorithm>
 #include <vector>
@@ -43,45 +43,30 @@ extern "C" {
 
 int sb_tta_decode_frames(const void* buf, int64_t nbytes, const int64_t* offsets, const int64_t* file_offsets, int64_t n,
                          const int32_t* config, sb_pcm** out) {
+    const char* who = "sb_tta_decode_frames";
     Ctx& c = ctx();
-    if (!c.inited) SB_FAIL(SB_ESTATE, "sb_tta_decode_frames: library not initialised (call sb_init)");
-    if (!buf || !offsets || !file_offsets || !config || !out) SB_FAIL(SB_EINVAL, "sb_tta_decode_frames: NULL argument");
+    SB_TRY(entry_check(who, buf && offsets && file_offsets && config && out));
     sbtta::Config cfg;
-    cfg.channels = config[0]; cfg.bits = config[1];
-    const int32_t rate = config[2];
-    cfg.frame_length = config[3]; cfg.last_length = config[4];
-    if (cfg.channels < 1 || cfg.channels > sbtta::kMaxChannels)
-        SB_FAIL(SB_EINVAL, "TTA with %d channels is not supported (1 to 8)", cfg.channels);
-    if (cfg.bits != 16 && cfg.bits != 24) SB_FAIL(SB_EINVAL, "TTA with %d bits per sample is not supported (16 or 24)", cfg.bits);
-    if (rate < 1 || rate > 0x7FFFFF || cfg.frame_length != (int32_t)(256ll * rate / 245) || cfg.frame_length < 1 ||
-        cfg.last_length < 0 || cfg.last_length >= cfg.frame_length || nbytes < 1 || n < 1)
-        SB_FAIL(SB_EINVAL, "sb_tta_decode_frames: bad stream parameters");
-    std::vector<sbtta::Frame> frames((size_t)n);
-    for (int64_t f = 0; f < n; ++f) {
-        const int64_t end = f + 1 < n ? offsets[f + 1] : nbytes;
-        if (offsets[f] < 0 || offsets[f] >= nbytes || end <= offsets[f] || end > nbytes)
-            SB_FAIL(SB_EINVAL, "TTA frame %lld at byte offset %lld: %s", (long long)f, (long long)file_offsets[f],
-                    offsets[f] < 0 || offsets[f] >= nbytes ? "frame starts outside the buffer" : "empty frame");
-        sbtta::Frame& d = frames[(size_t)f];
-        d.offset = offsets[f]; d.size = end - offsets[f]; d.sample = f * (int64_t)cfg.frame_length;
-        d.last = f + 1 == n; d.pad = 0;
-    }
-    const int64_t samples = (n - 1) * (int64_t)cfg.frame_length + (cfg.last_length ? cfg.last_length : cfg.frame_length);
+    int32_t rate = 0;
+    char msg[256];
+    if (!sbtta::parse_config(config, &cfg, &rate, msg, sizeof(msg))) SB_FAIL(SB_EINVAL, "%s", msg);
+    if (nbytes < 1 || n < 1) SB_FAIL(SB_EINVAL, "sb_tta_decode_frames: bad stream parameters");
+    std::vector<sbtta::Frame> frames;
+    int64_t samples = 0;
+    if (!sbtta::frame_table(offsets, file_offsets, n, nbytes, cfg, frames, &samples, msg, sizeof(msg)))
+        SB_FAIL(SB_EINVAL, "%s", msg);
+    Blocks blocks;
     uint8_t* d_buf = nullptr;
     sbtta::Frame* d_frames = nullptr;
     int16_t* d_pcm = nullptr;
     int32_t* d_status = nullptr;
-    auto release = [&]() { pool_free(d_buf); pool_free(d_frames); pool_free(d_status); };
-    auto fail = [&](int code) { release(); pool_free(d_pcm); return code; };
-    int rc = pool_alloc((void**)&d_buf, (size_t)nbytes + 16);
-    if (rc == SB_OK) rc = pool_alloc((void**)&d_frames, sizeof(sbtta::Frame) * n + 16);
-    if (rc == SB_OK) rc = pool_alloc((void**)&d_pcm, sizeof(int16_t) * (size_t)samples * cfg.channels + 16);
-    if (rc == SB_OK) rc = pool_alloc((void**)&d_status, sizeof(int32_t) * n + 16);
-    if (rc != SB_OK) return fail(rc);
+    SB_TRY(upload_padded(blocks, &d_buf, buf, nbytes, who));
+    SB_TRY(blocks.alloc(&d_frames, (size_t)n));
+    SB_TRY(blocks.alloc(&d_pcm, (size_t)samples * cfg.channels));
+    SB_TRY(blocks.alloc(&d_status, (size_t)n));
     std::vector<int32_t> status((size_t)n);
     const size_t smem = smem_bytes(cfg.channels);
     cudaError_t e = cudaFuncSetAttribute(k_tta_decode, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem);
-    if (e == cudaSuccess) e = cudaMemcpyAsync(d_buf, buf, (size_t)nbytes, cudaMemcpyHostToDevice, c.stream);
     if (e == cudaSuccess) e = cudaMemcpyAsync(d_frames, frames.data(), sizeof(sbtta::Frame) * n, cudaMemcpyHostToDevice,
                                               c.stream);
     if (e == cudaSuccess) {
@@ -90,17 +75,10 @@ int sb_tta_decode_frames(const void* buf, int64_t nbytes, const int64_t* offsets
                                                                                                 d_pcm, d_status);
         e = cudaGetLastError();
     }
-    if (e == cudaSuccess) e = cudaMemcpyAsync(status.data(), d_status, sizeof(int32_t) * n, cudaMemcpyDeviceToHost, c.stream);
-    if (e == cudaSuccess) e = cudaStreamSynchronize(c.stream);
-    if (e != cudaSuccess) { fail(0); SB_FAIL(SB_ECUDA, "sb_tta_decode_frames: %s", cudaGetErrorString(e)); }
-    for (int64_t f = 0; f < n; ++f)
-        if (status[(size_t)f] != sbtta::kOk) {
-            fail(0);
-            SB_FAIL(SB_EINVAL, "TTA frame %lld at byte offset %lld: %s", (long long)f, (long long)file_offsets[f],
-                    sbtta::error_text(status[(size_t)f]));
-        }
-    release();
-    return pcm_handle(d_pcm, samples, cfg.channels, rate, out);
+    SB_TRY(collect(e, status.data(), d_status, n, who));
+    if (!sbframes::first_failure(status.data(), n, "TTA frame", file_offsets, 1, sbtta::error_text, msg, sizeof(msg)))
+        SB_FAIL(SB_EINVAL, "%s", msg);
+    return pcm_handle(blocks.take(d_pcm), samples, cfg.channels, rate, out);
 }
 
 }  // extern "C"

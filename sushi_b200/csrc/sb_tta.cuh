@@ -15,6 +15,9 @@
 // the block's thread count), so the per-sample loop never touches local memory.
 #pragma once
 #include <stdint.h>
+#include <vector>
+
+#include "sb_frames.h"
 
 #if defined(__CUDACC__)
 #define SBT_HD __host__ __device__ __forceinline__
@@ -297,6 +300,45 @@ SBT_HD int decode_frame(const uint8_t* buf, const Frame& f, const Config& c, con
     const uint32_t stored = (uint32_t)q[0] | ((uint32_t)q[1] << 8) | ((uint32_t)q[2] << 16) | ((uint32_t)q[3] << 24);
     if (crc32(buf + f.offset, f.size - 4, crc_table) != stored) return kCrc;
     return kOk;
+}
+
+// ---- host side: what sb_tta_decode_frames does around the kernel; the CPU build of the tests runs the same ----
+
+// config[0..5) (channels, bits, rate, frame length, last frame length) into *c and *rate.  Returns false with a
+// message.
+inline bool parse_config(const int32_t* config, Config* c, int32_t* rate, char* msg, size_t msg_len) {
+    c->channels = config[0]; c->bits = config[1];
+    *rate = config[2];
+    c->frame_length = config[3]; c->last_length = config[4];
+    if (c->channels < 1 || c->channels > kMaxChannels)
+        snprintf(msg, msg_len, "TTA with %d channels is not supported (1 to 8)", c->channels);
+    else if (c->bits != 16 && c->bits != 24)
+        snprintf(msg, msg_len, "TTA with %d bits per sample is not supported (16 or 24)", c->bits);
+    else if (*rate < 1 || *rate > 0x7FFFFF || c->frame_length != (int32_t)(256ll * *rate / 245) || c->frame_length < 1 ||
+             c->last_length < 0 || c->last_length >= c->frame_length)
+        snprintf(msg, msg_len, "sb_tta_decode_frames: bad stream parameters");
+    else
+        return true;
+    return false;
+}
+
+// The kernel's frames: frame f holds bytes [offsets[f], offsets[f + 1]) of the buffer, the last up to nbytes, and
+// starts at sample f * frame_length.  Every frame must start inside the buffer, hold a byte and end inside it; `where`
+// names each frame's file offset.  *samples: the track's length.  Returns false with a message.
+inline bool frame_table(const int64_t* offsets, const int64_t* where, int64_t n, int64_t nbytes, const Config& c,
+                        std::vector<Frame>& frames, int64_t* samples, char* msg, size_t msg_len) {
+    frames.resize((size_t)n);
+    for (int64_t f = 0; f < n; ++f) {
+        const int64_t end = f + 1 < n ? offsets[f + 1] : nbytes;
+        if (offsets[f] < 0 || offsets[f] >= nbytes)
+            return sbframes::refuse(msg, msg_len, "TTA frame", f, where[f], "frame starts outside the buffer");
+        if (end <= offsets[f] || end > nbytes) return sbframes::refuse(msg, msg_len, "TTA frame", f, where[f], "empty frame");
+        Frame& d = frames[(size_t)f];
+        d.offset = offsets[f]; d.size = end - offsets[f]; d.sample = f * (int64_t)c.frame_length;
+        d.last = f + 1 == n; d.pad = 0;
+    }
+    *samples = (n - 1) * (int64_t)c.frame_length + (c.last_length ? c.last_length : c.frame_length);
+    return true;
 }
 
 }  // namespace sbtta

@@ -7,7 +7,7 @@
 //                      in a column of shared memory; nothing is kept per block in global scratch, so every block goes in
 //                      one launch.
 // The per-block arithmetic is in sb_wavpack.cuh, shared with the CPU emulation of the tests.
-#include "sb_internal.h"
+#include "sb_decode.h"
 #include "sb_wavpack.cuh"
 #include <algorithm>
 #include <vector>
@@ -37,42 +37,26 @@ extern "C" {
 
 int sb_wavpack_decode_blocks(const void* buf, int64_t nbytes, const int64_t* table, int64_t n, int32_t channels,
                              int32_t rate, sb_pcm** out) {
+    const char* who = "sb_wavpack_decode_blocks";
     Ctx& c = ctx();
-    if (!c.inited) SB_FAIL(SB_ESTATE, "sb_wavpack_decode_blocks: library not initialised (call sb_init)");
-    if (!buf || !table || !out) SB_FAIL(SB_EINVAL, "sb_wavpack_decode_blocks: NULL argument");
+    SB_TRY(entry_check(who, buf && table && out));
     if (channels < 1 || channels > 8) SB_FAIL(SB_EINVAL, "WavPack with %d channels is not supported (1 to 8)", channels);
     if (rate < 1 || nbytes < 1 || n < 1) SB_FAIL(SB_EINVAL, "sb_wavpack_decode_blocks: bad stream parameters");
-    std::vector<sbwv::Block> blocks((size_t)n);
+    std::vector<sbwv::Block> blocks_h;
     int64_t samples = 0;
-    for (int64_t i = 0; i < n; ++i) {
-        const int64_t* r = table + 8 * i;
-        sbwv::Block& b = blocks[(size_t)i];
-        b.offset = r[0]; b.size = r[1]; b.samples = (int32_t)r[2]; b.flags = (uint32_t)r[3]; b.crc = (uint32_t)r[4];
-        b.sample = r[5]; b.channel = (int32_t)r[6];
-        const int width = (b.flags & sbwv::kMono) ? 1 : 2;
-        if (r[0] < 0 || r[1] < 0 || r[0] > nbytes - r[1] || r[2] < 1 || r[2] > sbwv::kMaxBlockSamples || r[5] < 0 ||
-            r[6] < 0 || r[6] + width > channels)
-            SB_FAIL(SB_EINVAL, "WavPack block %lld at byte offset %lld: block table entry out of range", (long long)i,
-                    (long long)r[7]);
-        samples = std::max(samples, r[5] + r[2]);
-    }
+    char msg[256];
+    if (!sbwv::block_table(table, n, nbytes, channels, blocks_h, &samples, msg, sizeof(msg))) SB_FAIL(SB_EINVAL, "%s", msg);
+    Blocks blocks;
     uint8_t* d_buf = nullptr;
     sbwv::Block* d_blocks = nullptr;
     int16_t* d_pcm = nullptr;
     int32_t* d_status = nullptr;
-    auto release = [&]() { pool_free(d_buf); pool_free(d_blocks); pool_free(d_status); };
-    auto fail = [&](int code) { release(); pool_free(d_pcm); return code; };
-    int rc = pool_alloc((void**)&d_buf, (size_t)nbytes + 16);
-    if (rc == SB_OK) rc = pool_alloc((void**)&d_blocks, sizeof(sbwv::Block) * n + 16);
-    if (rc == SB_OK) rc = pool_alloc((void**)&d_pcm, sizeof(int16_t) * (size_t)samples * channels + 16);
-    if (rc == SB_OK) rc = pool_alloc((void**)&d_status, sizeof(int32_t) * n + 16);
-    if (rc != SB_OK) return fail(rc);
+    SB_TRY(upload_padded(blocks, &d_buf, buf, nbytes, who));
+    SB_TRY(blocks.alloc(&d_blocks, (size_t)n));
+    SB_TRY(blocks.alloc(&d_pcm, (size_t)samples * channels));
+    SB_TRY(blocks.alloc(&d_status, (size_t)n));
     std::vector<int32_t> status((size_t)n);
-    // the bit reader fetches 5 bytes at a time: zeros past the last block
-    cudaError_t e = cudaMemsetAsync(d_buf + nbytes, 0, 16, c.stream);
-    if (e == cudaSuccess) e = cudaMemcpyAsync(d_buf, buf, (size_t)nbytes, cudaMemcpyHostToDevice, c.stream);
-    if (e == cudaSuccess) e = cudaMemcpyAsync(d_blocks, blocks.data(), sizeof(sbwv::Block) * n, cudaMemcpyHostToDevice,
-                                              c.stream);
+    cudaError_t e = cudaMemcpyAsync(d_blocks, blocks_h.data(), sizeof(sbwv::Block) * n, cudaMemcpyHostToDevice, c.stream);
     if (e == cudaSuccess) e = cudaMemsetAsync(d_pcm, 0, sizeof(int16_t) * (size_t)samples * channels, c.stream);
     if (e == cudaSuccess) {
         ProfScope ps("wavpack_decode");
@@ -80,17 +64,10 @@ int sb_wavpack_decode_blocks(const void* buf, int64_t nbytes, const int64_t* tab
             d_buf, d_blocks, n, channels, d_pcm, d_status);
         e = cudaGetLastError();
     }
-    if (e == cudaSuccess) e = cudaMemcpyAsync(status.data(), d_status, sizeof(int32_t) * n, cudaMemcpyDeviceToHost, c.stream);
-    if (e == cudaSuccess) e = cudaStreamSynchronize(c.stream);
-    if (e != cudaSuccess) { fail(0); SB_FAIL(SB_ECUDA, "sb_wavpack_decode_blocks: %s", cudaGetErrorString(e)); }
-    for (int64_t i = 0; i < n; ++i)
-        if (status[(size_t)i] != sbwv::kOk) {
-            fail(0);
-            SB_FAIL(SB_EINVAL, "WavPack block %lld at byte offset %lld: %s", (long long)i, (long long)table[8 * i + 7],
-                    sbwv::error_text(status[(size_t)i]));
-        }
-    release();
-    return pcm_handle(d_pcm, samples, channels, rate, out);
+    SB_TRY(collect(e, status.data(), d_status, n, who));
+    if (!sbframes::first_failure(status.data(), n, "WavPack block", table + 7, 8, sbwv::error_text, msg, sizeof(msg)))
+        SB_FAIL(SB_EINVAL, "%s", msg);
+    return pcm_handle(blocks.take(d_pcm), samples, channels, rate, out);
 }
 
 }  // extern "C"

@@ -17,6 +17,10 @@
 // block's thread count), so the per-sample loop over terms never touches local memory.
 #pragma once
 #include <stdint.h>
+#include <algorithm>
+#include <vector>
+
+#include "sb_frames.h"
 
 #if defined(__CUDACC__)
 #define SBW_HD __host__ __device__ __forceinline__
@@ -543,6 +547,30 @@ SBW_HD int decode_block(const uint8_t* buf, const Block& blk, int channels, cons
     }
     if (crc != blk.crc) return kCrc;
     return kOk;
+}
+
+// ---- host side: what sb_wavpack_decode_blocks does around the kernel; the CPU build of the tests runs the same ----
+
+// The kernel's blocks from the caller's table (8 int64 per block: offset, size, samples, flags, crc, sample position,
+// first channel, file offset): a block must lie inside the buffer, hold 1 to kMaxBlockSamples samples and write
+// channels the track has.  *samples: where the last block ends.  Returns false with a message naming the row's file
+// offset.
+inline bool block_table(const int64_t* table, int64_t n, int64_t nbytes, int channels, std::vector<Block>& blocks,
+                        int64_t* samples, char* msg, size_t msg_len) {
+    blocks.resize((size_t)n);
+    *samples = 0;
+    for (int64_t i = 0; i < n; ++i) {
+        const int64_t* r = table + 8 * i;
+        Block& b = blocks[(size_t)i];
+        b.offset = r[0]; b.size = r[1]; b.samples = (int32_t)r[2]; b.flags = (uint32_t)r[3]; b.crc = (uint32_t)r[4];
+        b.sample = r[5]; b.channel = (int32_t)r[6];
+        const int width = (b.flags & kMono) ? 1 : 2;
+        if (r[0] < 0 || r[1] < 0 || r[0] > nbytes - r[1] || r[2] < 1 || r[2] > kMaxBlockSamples || r[5] < 0 ||
+            r[6] < 0 || r[6] + width > channels)
+            return sbframes::refuse(msg, msg_len, "WavPack block", i, r[7], "block table entry out of range");
+        *samples = std::max(*samples, r[5] + r[2]);
+    }
+    return true;
 }
 
 }  // namespace sbwv

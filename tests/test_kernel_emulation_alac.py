@@ -18,7 +18,8 @@ from tests import mkv_alac_cases as mac
 ROOT = os.path.dirname(os.path.dirname(os.path.abspath(__file__)))
 EMU = os.path.join(ROOT, 'tests', 'emu')
 DRIVER = os.path.join(EMU, 'emu_alac_driver.cpp')
-HEADER = os.path.join(ROOT, 'sushi_b200', 'csrc', 'sb_alac.cuh')
+SOURCES = [DRIVER, os.path.join(EMU, 'emu_guard.h'), os.path.join(ROOT, 'sushi_b200', 'csrc', 'sb_alac.cuh'),
+           os.path.join(ROOT, 'sushi_b200', 'csrc', 'sb_frames.h')]
 CASES = ac.all_cases()
 BASE, DAMAGED = ac.damaged_cases()
 
@@ -26,7 +27,7 @@ BASE, DAMAGED = ac.damaged_cases()
 @pytest.fixture(scope='module')
 def emu():
     out = os.path.join(EMU, '_build', 'libsb_emu_alac.so')
-    if not os.path.exists(out) or os.path.getmtime(out) < max(os.path.getmtime(DRIVER), os.path.getmtime(HEADER)):
+    if not os.path.exists(out) or os.path.getmtime(out) < max(os.path.getmtime(p) for p in SOURCES):
         os.makedirs(os.path.dirname(out), exist_ok=True)
         subprocess.check_call(['g++', '-std=c++17', '-O2', '-Wall', '-Wno-unused-function', '-Wno-format-security',
                                '-I', os.path.join(ROOT, 'sushi_b200', 'csrc'), '-shared', '-fPIC', DRIVER, '-o', out])
@@ -77,6 +78,29 @@ def test_damaged_frame_is_refused_naming_frame_and_offset(emu, damaged):
     assert pcm is None
     assert err.startswith('ALAC frame %d at byte offset %d: ' % (f, where[f])), err
     assert re.search(regex, err), err
+
+
+def test_frame_table_and_config_are_refused_in_the_library_s_words(emu):
+    """What sb_alac_decode_frames refuses before any kernel runs, through the same functions: a frame that starts
+    outside the buffer, an empty frame, and a config out of range."""
+    data, offsets, where = BASE.data, np.array(BASE.offsets, np.int64), np.array(BASE.offsets, np.int64) * 3 + 77
+    assert len(offsets) > 2
+    outside = offsets.copy()
+    outside[-1] = len(data)
+    assert decode(emu, data, outside, where, BASE.cfg) == (
+        None, 'ALAC frame %d at byte offset %d: frame starts outside the buffer' % (len(offsets) - 1, where[-1]))
+    outside[0] = -1
+    assert decode(emu, data, outside, where, BASE.cfg) == (
+        None, 'ALAC frame 0 at byte offset %d: frame starts outside the buffer' % where[0])
+    empty = offsets.copy()
+    empty[2] = empty[1]
+    assert decode(emu, data, empty, where, BASE.cfg) == (None, 'ALAC frame 1 at byte offset %d: empty frame' % where[1])
+    for field, value, text in (('bit_depth', 12, 'ALAC with 12 bits per sample is not supported (16, 20, 24 or 32)'),
+                               ('frame_length', 65537, 'ALAC frameLength 65537 is not supported (1 to 65536)'),
+                               ('channels', 9, 'ALAC with 9 channels is not supported (1 to 8)'),
+                               ('rate', 0, 'sb_alac_decode_frames: bad stream parameters')):
+        cfg = ac.Config(**dict(vars(BASE.cfg), **{field: value}))
+        assert decode(emu, data, offsets, where, cfg) == (None, text)
 
 
 GUARDED = r"""

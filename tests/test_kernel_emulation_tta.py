@@ -20,7 +20,8 @@ from tests import tta_cases as tc
 ROOT = os.path.dirname(os.path.dirname(os.path.abspath(__file__)))
 EMU = os.path.join(ROOT, 'tests', 'emu')
 DRIVER = os.path.join(EMU, 'emu_tta_driver.cpp')
-HEADER = os.path.join(ROOT, 'sushi_b200', 'csrc', 'sb_tta.cuh')
+SOURCES = [DRIVER, os.path.join(EMU, 'emu_guard.h'), os.path.join(ROOT, 'sushi_b200', 'csrc', 'sb_tta.cuh'),
+           os.path.join(ROOT, 'sushi_b200', 'csrc', 'sb_frames.h')]
 LIB = os.path.join(EMU, '_build', 'libsb_emu_tta.so')
 CASES = tc.all_cases()
 BASE, DAMAGED = tc.damaged_cases()
@@ -29,7 +30,7 @@ KERNEL = [d for d in DAMAGED if d[4]]
 
 @pytest.fixture(scope='module')
 def emu():
-    if not os.path.exists(LIB) or os.path.getmtime(LIB) < max(os.path.getmtime(DRIVER), os.path.getmtime(HEADER)):
+    if not os.path.exists(LIB) or os.path.getmtime(LIB) < max(os.path.getmtime(p) for p in SOURCES):
         os.makedirs(os.path.dirname(LIB), exist_ok=True)
         subprocess.check_call(['g++', '-std=c++17', '-O2', '-Wall', '-Wno-unused-function', '-Wno-format-security',
                                '-I', os.path.join(ROOT, 'sushi_b200', 'csrc'), '-shared', '-fPIC', DRIVER, '-o', LIB])
@@ -102,6 +103,28 @@ def test_host_refusals_come_before_the_decoder(tmp_path, damaged):
         _tta(tmp_path, name, data)
     if frame is not None:
         assert 'TTA frame %d at byte offset ' % frame in str(e.value), str(e.value)
+
+
+def test_frame_table_and_config_are_refused_in_the_library_s_words(emu, tmp_path):
+    """What sb_tta_decode_frames refuses before the kernel runs, through the same functions: a frame that starts outside
+    the buffer, an empty frame, and a config out of range."""
+    case = [c for c in CASES if c.name == 'three24'][0]
+    f = _tta(tmp_path, case.name, case.tta())
+    offsets, where, config = np.array(f.offsets, np.int64), np.array(f.where, np.int64), np.array(f.config, np.int32)
+    outside = offsets.copy()
+    outside[-1] = len(f.audio)
+    assert decode(emu, f.audio, outside, where, config) == (
+        None, 'TTA frame %d at byte offset %d: frame starts outside the buffer' % (len(offsets) - 1, where[-1]))
+    empty = offsets.copy()
+    empty[1] = empty[0]
+    assert decode(emu, f.audio, empty, where, config) == (None, 'TTA frame 0 at byte offset %d: empty frame' % where[0])
+    for index, value, text in ((0, 9, 'TTA with 9 channels is not supported (1 to 8)'),
+                               (1, 20, 'TTA with 20 bits per sample is not supported (16 or 24)'),
+                               (3, int(config[3]) + 1, 'sb_tta_decode_frames: bad stream parameters'),
+                               (4, int(config[3]), 'sb_tta_decode_frames: bad stream parameters')):
+        bad = config.copy()
+        bad[index] = value
+        assert decode(emu, f.audio, offsets, where, bad) == (None, text)
 
 
 def test_cut_frames_read_nothing_past_their_bytes(emu, tmp_path):

@@ -21,7 +21,8 @@ from tests import wavpack_cases as wc
 ROOT = os.path.dirname(os.path.dirname(os.path.abspath(__file__)))
 EMU = os.path.join(ROOT, 'tests', 'emu')
 DRIVER = os.path.join(EMU, 'emu_wavpack_driver.cpp')
-HEADER = os.path.join(ROOT, 'sushi_b200', 'csrc', 'sb_wavpack.cuh')
+SOURCES = [DRIVER, os.path.join(EMU, 'emu_guard.h'), os.path.join(ROOT, 'sushi_b200', 'csrc', 'sb_wavpack.cuh'),
+           os.path.join(ROOT, 'sushi_b200', 'csrc', 'sb_frames.h')]
 LIB = os.path.join(EMU, '_build', 'libsb_emu_wavpack.so')
 CASES = wc.all_cases()
 BASE, DAMAGED = wc.damaged_cases()
@@ -30,7 +31,7 @@ KERNEL = [d for d in DAMAGED if d[4]]
 
 @pytest.fixture(scope='module')
 def emu():
-    if not os.path.exists(LIB) or os.path.getmtime(LIB) < max(os.path.getmtime(DRIVER), os.path.getmtime(HEADER)):
+    if not os.path.exists(LIB) or os.path.getmtime(LIB) < max(os.path.getmtime(p) for p in SOURCES):
         os.makedirs(os.path.dirname(LIB), exist_ok=True)
         subprocess.check_call(['g++', '-std=c++17', '-O2', '-Wall', '-Wno-unused-function', '-Wno-format-security',
                                '-I', os.path.join(ROOT, 'sushi_b200', 'csrc'), '-shared', '-fPIC', DRIVER, '-o', LIB])
@@ -101,6 +102,25 @@ def test_host_refusals_come_before_the_decoder(tmp_path, damaged):
         _wv(tmp_path, name, data)
     if block is not None and 'is WavPack (' not in str(e.value):
         assert 'WavPack block %d at byte offset ' % block in str(e.value), str(e.value)
+
+
+@pytest.mark.parametrize('column,value', [(5, -1), (6, -1), (2, 150001), (2, 0), (0, -1), (1, -1), (1, 1 << 40), (6, 7)],
+                         ids=lambda v: str(v))
+def test_block_table_row_out_of_range_is_refused_naming_its_file_offset(emu, tmp_path, column, value):
+    """The rows sb_wavpack_decode_blocks refuses before the kernel runs, through the same function: a negative sample
+    position or channel, more samples than a block may hold, a block outside the buffer, a channel the track lacks."""
+    case = CASES[0]
+    f = _wv(tmp_path, case.name, case.wv())
+    table = np.array(f.table, np.int64)
+    row = len(table) - 1
+    table[row, column] = value
+    frames = int((f.table[:, 5] + f.table[:, 2]).max())
+    pcm = np.zeros((frames + 1, 8), np.int16)
+    msg = ctypes.create_string_buffer(256)
+    buf = np.frombuffer(f.data + bytes(16), np.uint8)
+    assert emu.emu_wavpack_decode(_p(buf), len(f.data), _p(table), len(table), case.channels, frames, _p(pcm), msg, 256) == -1
+    assert msg.value.decode() == 'WavPack block %d at byte offset %d: block table entry out of range' % (row, table[row, 7])
+    assert not pcm.any()
 
 
 def test_damaged_blocks_read_nothing_past_the_padding(emu, tmp_path):
