@@ -7,6 +7,9 @@ oracle/ and is test infrastructure only.
 import ctypes
 import os
 
+import numpy as np
+
+from ._nvtx import nvtx_range
 from .common import SushiError
 
 _HERE = os.path.dirname(os.path.abspath(__file__))
@@ -152,9 +155,27 @@ def bound_device():
     return _device
 
 
+def decode(device, name, *args):
+    """The sb_pcm handle a decoder entry point returns through its last argument.  The library is loaded here, so a
+    caller's host refusals come first."""
+    l = lib(device)
+    h = c_vp()
+    with nvtx_range('sushi_b200: ' + name):
+        check(getattr(l, name)(*args, ctypes.byref(h)), name)
+    return h
+
+
+def decode_frames(device, name, data, offsets, blocks, *args):
+    """decode of frames listed in `data`: frame f starts at offsets[f]; blocks[f] is the file offset errors name."""
+    buf = np.frombuffer(data + b'\0', dtype=np.uint8)          # never empty
+    offsets = np.ascontiguousarray(offsets, np.int64)
+    blocks = np.ascontiguousarray(blocks, np.int64)
+    return decode(device, name, buf.ctypes.data_as(c_vp), len(data) or 1, offsets.ctypes.data_as(c_i64p),
+                  blocks.ctypes.data_as(c_i64p), len(offsets), *args)
+
+
 def pinned_empty(shape, dtype):
     """numpy array over page-locked host memory (freed when the array is garbage collected)."""
-    import numpy as np
     import weakref
     l = lib()
     dt = np.dtype(dtype)

@@ -1,11 +1,9 @@
 """The Sushi command line: `python -m sushi_b200 --src a.mkv --dst b.mkv -o out.ass`.
 
-Flags, defaults and checks are the reference's (sushi.py:528-843).  --src and --dst are WAV, FLAC, WavPack (.wv),
-TTA (.tta), Matroska (.mkv, .mka, .mks, .webm), MP4 / QuickTime (.mp4, .m4a, .m4v, .mov) or transport stream files.
-For a WAV file the reference starts no subprocess either; a FLAC, WavPack or TTA file, a Matroska file's FLAC, ALAC,
-WavPack, TTA or PCM track, an MP4 file's ALAC, FLAC or PCM track, or a transport stream's (.m2ts, .mts, .m2t, .ts)
-BD-LPCM or TrueHD stream, is decoded on the GPU, where the reference would have ffmpeg convert it to a WAV file
-(DESIGN.md section 2): no WAV file is ever written.  A Matroska input also gives, as the reference's ffmpeg and
+Flags, defaults and checks are the reference's (sushi.py:528-843).  --src and --dst are files of the formats in
+inputs.FORMATS, taken by their extensions.  For a WAV file the reference starts no subprocess either; any other
+format is decoded on the GPU, where the reference would have ffmpeg convert it to a WAV file (DESIGN.md section 2):
+no WAV file is ever written.  A Matroska input also gives, as the reference's ffmpeg and
 mkvextract calls do, the script, the chapters and the video timestamps (sushi_b200.matroska); those are written to
 the reference's temporary paths and removed at the end unless --no-cleanup is given.  Every check runs before the GPU
 is touched; the run itself is pipeline.shift_script.
@@ -18,13 +16,11 @@ import sys
 import time
 
 from . import __version__
-from . import matroska, mp4, mpegts, tta, wavpack
 from .common import SushiError
+from .inputs import FORMATS
 from .pipeline import shift_script
 from .script import format_srt_time
 from .timing import get_ogm_start_times, get_xml_start_times, load_keyframe_times
-
-MATROSKA_EXTENSIONS = ('.mkv', '.mka', '.mks', '.webm')
 
 
 def get_extension(path):
@@ -123,51 +119,28 @@ def create_arg_parser():
 
 
 def _open_input(path):
-    """None for a WAV, FLAC, raw TrueHD (.thd), raw WavPack (.wv) or raw TTA (.tta) input; the opened MatroskaFile for a Matroska one, the opened
-    TransportStream for a transport stream (.m2ts, .mts, .m2t, .ts).  Anything else, or a Matroska or transport stream
-    name that does not open as one, is refused where the reference would have ffmpeg demux it."""
+    """The opened reader of a container input (inputs.FORMATS: Matroska, MP4, transport stream), which also gives its
+    script, chapters and streams; None for a WAV, FLAC, raw TrueHD (.thd), raw WavPack (.wv) or raw TTA (.tta) input,
+    which WavStream reads.  Any other extension, or a container's that does not open as one, is refused where the
+    reference would have ffmpeg demux it."""
     ext = get_extension(path)
-    if ext in wavpack.WV_EXTENSIONS:
-        wavpack.WavPackFile(path)                  # its refusals, before the GPU is touched
+    fmt = next((f for f in FORMATS if ext in f.extensions), None)
+    refusal = '{0}: demuxing is not supported, convert the input to WAV or FLAC first'.format(path)
+    if fmt is None:
+        raise SushiError(refusal)
+    if fmt.opens_as is None:
+        if fmt.name in ('WavPack', 'TTA'):
+            fmt.reader(path)                       # its refusals, before the GPU is touched
         return None
-    if ext in tta.TTA_EXTENSIONS:
-        tta.TTAFile(path)                          # its refusals, before the GPU is touched
-        return None
-    if ext in ('.wav', '.flac', '.thd'):
-        return None
-    if ext in mpegts.TS_EXTENSIONS:
-        try:
-            return mpegts.TransportStream(path)
-        except (OSError, SushiError) as e:
-            raise SushiError('{0}: demuxing is not supported, convert the input to WAV or FLAC first '
-                             '(it does not open as a transport stream: {1})'.format(path, e))
-    if ext in MATROSKA_EXTENSIONS:
-        try:
-            return matroska.MatroskaFile(path)
-        except (OSError, SushiError) as e:
-            raise SushiError('{0}: demuxing is not supported, convert the input to WAV or FLAC first '
-                             '(it does not open as a Matroska file: {1})'.format(path, e))
-    if ext in mp4.MP4_EXTENSIONS:
-        try:
-            return mp4.Mp4File(path)
-        except (OSError, SushiError) as e:
-            raise SushiError('{0}: demuxing is not supported, convert the input to WAV or FLAC first '
-                             '(it does not open as an MP4 file: {1})'.format(path, e))
-    raise SushiError('{0}: demuxing is not supported, convert the input to WAV or FLAC first'.format(path))
+    try:
+        return fmt.reader(path)
+    except (OSError, SushiError) as e:
+        raise SushiError('{0} (it does not open as {1}: {2})'.format(refusal, fmt.opens_as, e))
 
 
-def _select_audio(mkv, idx):
-    """The stream id of a Matroska or transport stream input's audio track (None for WAV and FLAC), refusing what
-    cannot be decoded."""
-    if mkv is None:
-        return None
-    track = mkv.select('audio', idx)
-    if isinstance(mkv, mp4.Mp4File):
-        mp4.audio_codec(track)
-        mkv.check_edits(track)
-    else:
-        (mpegts if isinstance(mkv, mpegts.TransportStream) else matroska).audio_codec(track)
-    return track.id
+def _select_audio(reader, idx):
+    """The stream id of a container input's audio track (None for the other inputs), refusing what cannot be decoded."""
+    return None if reader is None else reader.select_audio(idx).id
 
 
 def run(args):
@@ -285,12 +258,9 @@ def _run(args, ignore_chapters, src_mkv, dst_mkv, written):
                 return external_file
             if fps_arg:
                 return None
-            if isinstance(mkv, mpegts.TransportStream):
-                raise SushiError('{0}: video timestamps cannot be read from a transport stream here; pass --src-fps / '
-                                 '--dst-fps or a timecodes file'.format(path))
-            if isinstance(mkv, mp4.Mp4File):
-                raise SushiError('{0}: video timestamps cannot be read from an MP4 file here; pass --src-fps / '
-                                 '--dst-fps or a timecodes file'.format(path))
+            if mkv is not None and mkv.no_timecodes:
+                raise SushiError('{0}: video timestamps cannot be read from {1} here; pass --src-fps / --dst-fps or a '
+                                 'timecodes file'.format(path, mkv.no_timecodes))
             if mkv is not None and mkv.streams('video'):
                 out = format_full_path(args.temp_dir, path, '.sushi.timecodes.txt')
                 extract.append((out, mkv.timecodes_text))

@@ -1,11 +1,20 @@
 """Small helpers shared by the host side (mirror of the pieces of the reference's
 common.py that the hot path touches: SushiError common.py:4, clip common.py:41-42,
 format_time common.py:32-38 -- used only in log lines)."""
+import collections
 import logging
 
 
 class SushiError(Exception):
     """User-facing failure; the reference's CLI prints it and exits 2 (sushi.py:841-843)."""
+
+
+# What every reader's select_audio(track) returns, once each refusal that needs no GPU has passed: the audio WavStream
+# loads.  `label` names a codec the GPU decodes ('FLAC', 'TrueHD', 'BD-LPCM', ...) and is None for PCM; `id` is the
+# stream id in a container; `path` names the file in messages.  A codec has decode(device) -> the sb_pcm handle of the
+# decoded samples (it loads the library, and reads a container track's frames first) and may have check(frames), which
+# refuses the decoded frame count; PCM has pcm() -> (bytes, frames, channels, sample width, rate, big-endian).
+Audio = collections.namedtuple('Audio', 'label id path decode pcm check', defaults=(None,) * 5)
 
 
 def clip(value, minimum, maximum):

@@ -1,0 +1,35 @@
+"""The input formats, in one table.  Each has a host-side reader in its own module (this is the only module that knows
+them all) with one method, select_audio(track=None), which makes every refusal that needs no GPU and returns the
+common.Audio WavStream loads.  WavStream detects the format (open_input); the command line goes by file extension."""
+import collections
+
+from . import matroska, mp4, mpegts, truehd, tta, wavpack
+from .flac import FlacFile, is_flac
+from .wav import DownmixedWavFile
+
+# name: as the log names it; extensions: what the command line takes it by; sniff(path): whether a file is one (by its
+# content; a transport stream and a TrueHD stream by its name), asked in the table's order; reader: its class; opens_as:
+# for a container, whose script, chapters and streams the command line reads too, what its extensions must open as.
+Format = collections.namedtuple('Format', 'name extensions sniff reader opens_as')
+FORMATS = (
+    Format('transport stream', mpegts.TS_EXTENSIONS, mpegts.is_transport_stream, mpegts.TransportStream,
+           'a transport stream'),
+    Format('MP4', mp4.MP4_EXTENSIONS, mp4.is_mp4, mp4.Mp4File, 'an MP4 file'),
+    Format('Matroska', matroska.MATROSKA_EXTENSIONS, matroska.is_matroska, matroska.MatroskaFile, 'a Matroska file'),
+    Format('TrueHD', truehd.THD_EXTENSIONS, truehd.is_truehd, truehd.TrueHDFile, None),
+    Format('WavPack', wavpack.WV_EXTENSIONS, wavpack.is_wavpack, wavpack.WavPackFile, None),
+    Format('TTA', tta.TTA_EXTENSIONS, tta.is_tta, tta.TTAFile, None),
+    Format('FLAC', ('.flac',), is_flac, FlacFile, None),
+    Format('WAV', ('.wav',), lambda path: True, DownmixedWavFile, None),      # whatever is nothing else
+)
+
+
+def open_input(source):
+    """(reader, format name) of `source`: a file name, whose format is detected by content, or an opened container
+    reader (MatroskaFile, Mp4File, TransportStream), which is returned as it is and never sniffed."""
+    for f in FORMATS:
+        if f.opens_as and isinstance(source, f.reader):
+            return source, f.name
+    for f in FORMATS:
+        if f.sniff(source):
+            return f.reader(source), f.name

@@ -24,9 +24,10 @@ import zlib
 
 import numpy as np
 
-from . import tta, wavpack
-from .common import SushiError, py2_round, select_stream
+from . import _native, alac, flac, truehd, tta, wavpack
+from .common import Audio, SushiError, py2_round, select_stream
 
+MATROSKA_EXTENSIONS = ('.mkv', '.mka', '.mks', '.webm')
 EBML_MAGIC = b'\x1a\x45\xdf\xa3'
 
 # element ids, marker bits included
@@ -187,6 +188,30 @@ class FrameTable(object):
 
     def frame(self, i):
         return self.data[self.offset[i]:self.offset[i] + self.size[i]]
+
+
+def track_audio(path, track_id, label, read_frames, decode):
+    """The Audio of a container's audio track of the codec `label`: it loads exactly as the plain PCM WAV of the
+    samples FFmpeg's decoder returns, frames concatenated in container order (timestamp gaps are not filled).  The
+    order of what can refuse it: the caller has made the track's own refusals (selection, codec, edits, a FLAC track's
+    metadata and bit depth, TTA's config); WavStream refuses the host loader; then, in the Audio's decode, read_frames()
+    reads the track's FrameTable, an empty frame is refused, and decode(device, table) does what host work the frames
+    need (WavPack's block table), loads the library and decodes the frames on the GPU where the table puts them,
+    errors naming the file offset of a frame's block."""
+    def run(device):
+        table = read_frames()
+        table.refuse_empty(path, label)
+        return decode(device, table)
+    return Audio(label, track_id, path, decode=run)
+
+
+def track_pcm(path, track_id, read_frames, channels, rate, width, big_endian):
+    """The Audio of a container's integer PCM track: the whole sample frames of its FrameTable's bytes."""
+    def pcm():
+        data = read_frames().data
+        frames = len(data) // (channels * width)
+        return data[:frames * channels * width], frames, channels, width, rate, big_endian
+    return Audio(None, track_id, path, pcm=pcm)
 
 
 class _Source(object):
@@ -651,7 +676,40 @@ class MatroskaFile(object):
         """The reference's Demuxer._select_stream (demux.py:335-355): kind is 'audio', 'subtitles' or 'video'."""
         return select_stream(self.streams(kind), kind, idx, self.path)
 
+    def select_audio(self, track=None):
+        """The audio track `track` (a stream id; None: the reference's default rule).  Its table is released from this
+        file once read."""
+        t = self.select('audio', track)
+        kind = audio_codec(t)
+        name = '{0} track {1}'.format(self.path, t.id)
+
+        def read_frames():
+            table = self.frames([t.id])[t.id]
+            self.release([t.id])
+            return table
+
+        def decode_truehd(device, table):
+            _native.lib(device)                     # a missing library or GPU is reported before the major sync is read
+            truehd.MajorSync(table.data[:64], name)
+            return truehd.decode(device, table.data, table.offset, table.block)
+        if kind == 'pcm':
+            return track_pcm(self.path, t.id, read_frames, t.channels, int(t.sampling_frequency), t.bit_depth // 8,
+                             False)
+        if kind == 'flac':
+            label, decode = 'FLAC', flac.track_decoder(t.codec_private, name)
+        elif kind == 'alac':
+            label, decode = 'ALAC', alac.track_decoder(t.codec_private)
+        elif kind == 'wavpack':
+            label, decode = 'WavPack', wavpack.track_decoder(t)
+        elif kind == 'tta':
+            label, decode = 'TTA', tta.track_decoder(t, self.timestamp_scale, self.duration)
+        else:
+            label, decode = 'TrueHD', decode_truehd
+        return track_audio(self.path, t.id, label, read_frames, decode)
+
     # -- side products ----------------------------------------------------------------------------------------------
+    no_timecodes = None                             # video timestamps can be read (timecodes_text)
+
     def script_text(self, track):
         """The script of a subtitle track as the file the reference's ffmpeg call writes: ASS / SSA as CodecPrivate
         and one Dialogue line per block in ReadOrder (times rounded to centiseconds), UTF-8 as numbered SRT entries

@@ -26,8 +26,9 @@ import struct
 
 import numpy as np
 
+from . import alac, flac
 from .common import SushiError, select_stream
-from .matroska import FrameTable
+from .matroska import FrameTable, track_audio, track_pcm
 
 MP4_EXTENSIONS = ('.mp4', '.m4a', '.m4v', '.mov')
 TOP_LEVEL = (b'ftyp', b'moov', b'mdat', b'free', b'skip', b'wide', b'uuid', b'pnot', b'meta', b'moof', b'mfra',
@@ -129,6 +130,7 @@ class Track(object):
 
 class Mp4File(object):
     """The box structure of an MP4 / QuickTime file."""
+    no_timecodes = 'an MP4 file'                # what the command line says video timestamps cannot be read from
 
     def __init__(self, path):
         self.path = path
@@ -483,6 +485,19 @@ class Mp4File(object):
     def select(self, kind, idx):
         """The reference's Demuxer._select_stream (demux.py:335-355), as MatroskaFile.select."""
         return select_stream(self.streams(kind), kind, idx, self.path)
+
+    def select_audio(self, track=None):
+        """The audio track `track` (a stream id; None: the reference's default rule)."""
+        t = self.select('audio', track)
+        kind = audio_codec(t)
+        self.check_edits(t)
+        if kind == 'pcm':
+            return track_pcm(self.path, t.id, lambda: self.frames(t), t.channels, t.rate, *PCM_DECODED[t.codec])
+        if kind == 'flac':
+            label, decode = 'FLAC', flac.track_decoder(t.config, '{0} track {1}'.format(self.path, t.id))
+        else:
+            label, decode = 'ALAC', alac.track_decoder(t.config)
+        return track_audio(self.path, t.id, label, lambda: self.frames(t), decode)
 
     def prefetch(self, payload_ids=(), time_ids=()):
         """Nothing to read ahead: the audio is read by WavStream, and there is no script or timestamp to read."""

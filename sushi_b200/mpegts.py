@@ -17,10 +17,15 @@ What is kept of FFmpeg's stream rules:
 Only the first PMT version is read: streams a later PMT announces are not listed.  Elementary-stream descriptors
 (languages, stream-level registrations) are not read.  A PAT listing more than one program is refused.
 """
+import ctypes
 import logging
 import os
 
-from .common import SushiError, select_stream
+import numpy as np
+
+from . import _native
+from ._nvtx import nvtx_range
+from .common import Audio, SushiError, select_stream
 
 TS_EXTENSIONS = ('.m2ts', '.mts', '.m2t', '.ts')
 PROBE_SIZE = 5000000             # FFmpeg's default probesize: the PAT and the PMT must lie in this many bytes
@@ -38,7 +43,7 @@ HDMV_TYPES = {0x80: ('audio', 'pcm_bluray'), 0x81: ('audio', 'ac3'), 0x82: ('aud
               0xA2: ('audio', 'dts'), 0x90: ('subtitles', 'hdmv_pgs_subtitle'),
               0x92: ('subtitles', 'hdmv_text_subtitle')}
 MISC_TYPES = {0x81: ('audio', 'ac3'), 0x8A: ('audio', 'dts')}
-DECODED = ('pcm_bluray', 'truehd')
+DECODED = {'pcm_bluray': ('BD-LPCM', _native.SB_TS_PCM_BLURAY), 'truehd': ('TrueHD', _native.SB_TS_TRUEHD)}
 
 
 def is_transport_stream(path):
@@ -77,6 +82,7 @@ class Stream(object):
 class TransportStream(object):
     """The head of a transport stream: packet size, program and stream list.  `chapters` is always empty (FFmpeg's
     mpegts demuxer gives none)."""
+    no_timecodes = 'a transport stream'         # what the command line says video timestamps cannot be read from
 
     def __init__(self, path):
         self.path = path
@@ -223,6 +229,34 @@ class TransportStream(object):
                 k += 1
                 if got < n:
                     return
+
+    def select_audio(self, track=None):
+        s = self.select('audio', track)
+        return Audio(DECODED[audio_codec(s)][0], s.id, self.path, decode=lambda device: self._decode(device, s))
+
+    def _decode(self, device, s):
+        """The BD-LPCM or TrueHD stream `s`, demuxed and decoded on the GPU (sb_ts_*).  The file is read in chunks of
+        CHUNK_BYTES into two page-locked buffers, one after the other, so that the GPU scans one chunk while the next
+        is read."""
+        lib = _native.lib(device)
+        t = ctypes.c_void_p()
+        _native.check(lib.sb_ts_open(self.packet_size, s.pid, DECODED[s.codec][1], ctypes.byref(t)), 'sb_ts_open')
+        cut = ctypes.c_int32()
+        try:
+            size = max(self.packet_size, CHUNK_BYTES // self.packet_size * self.packet_size)
+            buffers = [_native.pinned_empty((size,), np.uint8) for _ in range(2)]
+            with nvtx_range('sushi_b200: sb_ts_feed'):
+                for view, pos in self.chunks(buffers):
+                    arr = np.frombuffer(view, np.uint8)
+                    _native.check(lib.sb_ts_feed(t, arr.ctypes.data_as(ctypes.c_void_p), len(arr), pos), 'sb_ts_feed')
+            del buffers
+            h = _native.decode(device, 'sb_ts_finish', t, ctypes.byref(cut))
+        finally:
+            lib.sb_ts_destroy(t)
+        if cut.value:
+            logging.warning('{0}: the last PES packet of stream {1} is cut short; its whole sample frames are '
+                            'kept'.format(self.path, s.id))
+        return h
 
 
 def audio_codec(stream):

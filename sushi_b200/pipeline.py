@@ -95,9 +95,9 @@ def _resolve_links(events):
 
 def shift_script(src_audio, dst_audio, script_path, output_path, sample_rate=12000, sample_type='uint8',
                  chapter_times=(), src_track=None, dst_track=None, **options):
-    """src/dst WAV, FLAC or Matroska (a path, or an opened MatroskaFile) + ASS/SRT script in, shifted script out (the
-    audio-in/script-out core of the CLI).
-    src_track / dst_track are the audio stream ids of Matroska inputs (None: the reference's default rule).
+    """src/dst audio (whatever WavStream takes: a file of a format in inputs.FORMATS, or an opened container reader) +
+    ASS/SRT script in, shifted script out (the audio-in/script-out core of the CLI).
+    src_track / dst_track are the audio stream ids of container inputs (None: the reference's default rule).
     `options` are shift_events' keyword arguments, keyframes included."""
     script = load_script(script_path)
     script.sort_by_time()

@@ -1,7 +1,10 @@
 """Dolby TrueHD streams on the host: recognising a raw .thd file and reading its first major sync (sample rate, samples
 per access unit, substreams, the decoded presentation's channel count) for the refusals WavStream gives before the GPU
 is touched.  The decode itself, and every check of the stream, is sb_truehd_decode on the GPU."""
-from .common import SushiError
+import numpy as np
+
+from . import _native
+from .common import Audio, SushiError
 
 SYNC_TRUEHD = b'\xf8\x72\x6f\xba'
 SYNC_MLP = b'\xf8\x72\x6f\xbb'
@@ -47,10 +50,24 @@ def is_truehd(path):
     return str(path).lower().endswith(THD_EXTENSIONS + ('.mlp',))
 
 
-def read_stream(path):
-    """The file's bytes and its first major sync; an .mlp file is refused."""
-    if str(path).lower().endswith('.mlp'):
-        raise SushiError('{0}: MLP (DVD-Audio) is not supported, only Dolby TrueHD'.format(path))
-    with open(path, 'rb') as f:
-        data = f.read()
-    return data, MajorSync(data, path)
+class TrueHDFile(object):
+    """A raw TrueHD stream: the file's bytes and its first major sync; an .mlp file is refused."""
+
+    def __init__(self, path):
+        if str(path).lower().endswith('.mlp'):
+            raise SushiError('{0}: MLP (DVD-Audio) is not supported, only Dolby TrueHD'.format(path))
+        self.path = path
+        with open(path, 'rb') as f:
+            self.data = f.read()
+        self.sync = MajorSync(self.data, path)
+
+    def select_audio(self, track=None):
+        # one block holding every access unit; a negative file offset makes messages name each unit's own offset
+        return Audio('TrueHD', path=self.path, decode=lambda device: decode(
+            device, self.data, np.zeros(1, np.int64), np.full(1, -1, np.int64)))
+
+
+def decode(device, data, offsets, blocks):
+    """sb_truehd_decode on the blocks of access units at `offsets` in `data`; blocks[i] is the file offset errors
+    name."""
+    return _native.decode_frames(device, 'sb_truehd_decode', data, offsets, blocks)

@@ -9,13 +9,15 @@ bitstream and each frame's CRC are checked on the GPU.
 A frame table is the frames' bytes back to back, each frame's offset in them, the file offset errors name (the
 frame's own in a .tta file, its block's in a Matroska file), and the config sb_tta_decode_frames takes: channels, bits,
 rate, frame length (256 * rate / 245) and the last frame's length (0 for a whole frame)."""
+import ctypes
 import struct
 import zlib
 
 import numpy as np
 
-from . import wavpack, wavstream
-from .common import SushiError
+from . import _native, wavpack
+from .common import Audio, SushiError
+from .flac import id3v2_size
 
 TTA_EXTENSIONS = ('.tta',)
 MAX_RATE = 1000000                  # FFmpeg's tta demuxer refuses a higher rate
@@ -27,7 +29,7 @@ def is_tta(path):
     try:
         with open(path, 'rb') as f:
             head = f.read(10)
-            skip = wavstream.id3v2_size(head)
+            skip = id3v2_size(head)
             if skip:
                 f.seek(skip)
                 head = f.read(4)
@@ -76,7 +78,7 @@ class TTAFile(object):
         self.path = path
         with open(path, 'rb') as f:
             self.data = data = f.read()
-        at = wavstream.id3v2_size(data[:10])
+        at = id3v2_size(data[:10])
         if len(data) < at + 22 or data[at:at + 4] != b'TTA1':
             raise SushiError('{0}: not a TTA file'.format(path))
         _, fmt, channels, bits, rate, total, crc = _HEADER.unpack_from(data, at)
@@ -120,6 +122,16 @@ class TTAFile(object):
         self.offsets = starts - first
         self.where = starts
 
+    def select_audio(self, track=None):
+        return Audio('TTA', path=self.path, decode=self._decode)
+
+    def _decode(self, device):
+        # the file's bytes as read, up to the end of the audio: frames at their file offsets, no copy
+        buf = np.frombuffer(self.data, dtype=np.uint8)
+        where = self.where.ctypes.data_as(_native.c_i64p)
+        return _native.decode(device, 'sb_tta_decode_frames', buf.ctypes.data_as(ctypes.c_void_p), self.end, where,
+                              where, len(self.where), self.config.ctypes.data_as(_native.c_i32p))
+
 
 def check_track(track):
     """An A_TTA1 track's refusals, before any frame is read: FFmpeg builds its TTA header from the track (format 1,
@@ -146,3 +158,10 @@ def matroska_config(track, timestamp_scale, duration):
         ns = int(duration * timestamp_scale)            # the double product, truncated to int64
         total = ((ns * rate + 500000000) // 1000000000) & 0xFFFFFFFF
     return _config(track.channels, track.bit_depth, rate, total, 'Audio track {0}'.format(track.id))
+
+
+def track_decoder(track, timestamp_scale, duration):
+    """decode(device, table) of an A_TTA1 track (sb_tta_decode_frames on its FrameTable, with matroska_config)."""
+    config = matroska_config(track, timestamp_scale, duration)
+    return lambda device, table: _native.decode_frames(device, 'sb_tta_decode_frames', table.data, table.offset,
+                                                       table.block, config.ctypes.data_as(_native.c_i32p))

@@ -10,11 +10,13 @@ checked on the GPU.
 
 A block table has one row of 8 int64 per block: the offset and size of its sub-blocks in the uploaded bytes, block
 samples, flags, CRC, the track sample where it starts, its first output channel, and the file offset errors name."""
+import ctypes
 import struct
 
 import numpy as np
 
-from .common import SushiError
+from . import _native
+from .common import Audio, SushiError
 
 WV_EXTENSIONS = ('.wv',)
 VERSIONS = (0x402, 0x410)
@@ -227,6 +229,25 @@ class WavPackFile(object):
         if total != 0xFFFFFFFF and total != self.samples:
             raise SushiError('{0}: WavPack header says {1} samples, the blocks hold {2}'.format(path, total, self.samples))
         self.table = table
+
+    def select_audio(self, track=None):
+        return Audio('WavPack', path=self.path,
+                     decode=lambda device: decode(device, self.data, self.table, self.stream))
+
+
+def decode(device, data, table, stream):
+    """sb_wavpack_decode_blocks on the blocks of `table` (a block table, above) in `data`."""
+    buf = np.frombuffer(data, dtype=np.uint8)
+    table = np.ascontiguousarray(table, np.int64)
+    return _native.decode(device, 'sb_wavpack_decode_blocks', buf.ctypes.data_as(ctypes.c_void_p), len(data),
+                          table.ctypes.data_as(_native.c_i64p), len(table), stream.channels, stream.rate)
+
+
+def track_decoder(track):
+    """decode(device, table) of an A_WAVPACK4 track: matroska_table on its FrameTable (the stream version from
+    CodecPrivate, and the channel count a multi-block frame must code), then decode."""
+    return lambda device, table: decode(device, table.data, *matroska_table(table, track.codec_private, track.id,
+                                                                             track.channels))
 
 
 def matroska_table(table, codec_private, track_id, declared_channels):

@@ -14,22 +14,18 @@ sample conversions stay here, in Python, written exactly as the reference writes
 them, so the integer offsets handed to the library are bit-identical.
 """
 import ctypes
-import io
 import logging
 import math
-import os
-import struct
-import weakref
 from time import time
+import weakref
 
 import numpy as np
 
-from . import _native, matroska, mp4, mpegts, truehd, tta, wavpack
+from . import _native
 from ._nvtx import nvtx_range
 from .common import SushiError, clip, py2_round
-
-WAVE_FORMAT_PCM = 0x0001
-WAVE_FORMAT_EXTENSIBLE = 0xFFFE
+from .inputs import open_input, FlacFile, is_flac   # noqa: F401  (the FLAC reader stays importable from here)
+from .wav import DownmixedWavFile, decode_downmix, nearest_index_map, normalise_host   # noqa: F401
 
 _DTYPES = {'uint8': (np.uint8, _native.SB_U8), 'float32': (np.float32, _native.SB_F32)}
 
@@ -37,267 +33,6 @@ _DTYPES = {'uint8': (np.uint8, _native.SB_U8), 'float32': (np.float32, _native.S
 # get_substream / np.split return, sushi.py:417,445) is recognised and handed to the
 # GPU as an (offset, length) descriptor instead of being uploaded again.
 _live_streams = weakref.WeakSet()
-
-
-class DownmixedWavFile(object):
-    """RIFF/WAVE reader + int16/int24 decode + channel averaging (wav.py:15-101).
-
-    Header walking stays on the host (survey row a10); decode/downmix of the PCM
-    payload is done by ``readframes`` on the host for the streaming loader and by
-    the GPU loader kernels for whole-file loads.
-    """
-
-    def __init__(self, path):
-        self._file = open(path, 'rb')
-        self.channels_count = self.framerate = self.sample_width = self.frame_size = None
-        self.frames_count = None
-        try:
-            head = self._file.read(12)
-            if len(head) < 12 or head[0:4] != b'RIFF':
-                raise SushiError('File does not start with RIFF id')
-            if head[8:12] != b'WAVE':
-                raise SushiError('Not a WAVE file')
-            file_size = os.path.getsize(path)
-            have_fmt = have_data = False
-            while True:
-                hdr = self._file.read(8)
-                if len(hdr) < 8:
-                    break
-                name, size = hdr[0:4], struct.unpack('<L', hdr[4:8])[0]
-                if name == b'fmt ':
-                    self._read_fmt_chunk(self._file.read(size + (size & 1)))
-                    have_fmt = True
-                    continue
-                if name == b'data':
-                    if file_size > 0xFFFFFFFF:
-                        # >4 GiB "broken" wav: trust the file size, not the 32-bit chunk size (wav.py:42-44)
-                        self.frames_count = (file_size - self._file.tell()) // self.frame_size
-                    else:
-                        self.frames_count = size // self.frame_size
-                    self.data_offset = self._file.tell()
-                    have_data = True
-                    break
-                self._file.seek(size + (size & 1), os.SEEK_CUR)
-            if not have_fmt or not have_data:
-                raise SushiError('Invalid WAV file')
-        except Exception:
-            self.close()
-            raise
-
-    @classmethod
-    def from_bytes(cls, data, channels, framerate, sample_width):
-        """A reader over in-memory interleaved little-endian PCM, as if it were a WAV file's data chunk."""
-        self = cls.__new__(cls)
-        self._file = io.BytesIO(data)
-        self.channels_count, self.framerate, self.sample_width = channels, framerate, sample_width
-        self.frame_size = channels * sample_width
-        self.frames_count = len(data) // self.frame_size
-        return self
-
-    def __del__(self):
-        self.close()
-
-    def close(self):
-        f = getattr(self, '_file', None)
-        if f:
-            f.close()
-            self._file = None
-
-    def _read_fmt_chunk(self, payload):
-        tag, self.channels_count, self.framerate, _, _ = struct.unpack('<HHLLH', payload[:14])
-        if tag not in (WAVE_FORMAT_PCM, WAVE_FORMAT_EXTENSIBLE):
-            raise SushiError('unknown format: {0}'.format(tag))
-        bits = struct.unpack('<H', payload[14:16])[0]
-        self.sample_width = (bits + 7) // 8
-        self.frame_size = self.channels_count * self.sample_width
-
-    def read_raw(self, count):
-        return self._file.read(count * self.frame_size)
-
-    def readframes(self, count):
-        """Decode `count` frames to mono float32 (wav.py:64-91)."""
-        if not count:
-            return np.zeros(0, np.float32)
-        return decode_downmix(self.read_raw(count), self.sample_width, self.channels_count)
-
-
-FLAC_MAGIC = b'fLaC'
-FLAC_BLOCK_NAMES = {0: 'STREAMINFO', 1: 'PADDING', 2: 'APPLICATION', 3: 'SEEKTABLE', 4: 'VORBIS_COMMENT', 5: 'CUESHEET',
-                    6: 'PICTURE'}
-
-
-def id3v2_size(head):
-    """Bytes of an ID3v2 tag at the start of `head` (header, syncsafe size, optional footer), or 0 if there is none."""
-    if len(head) < 10 or head[0:3] != b'ID3':
-        return 0
-    size = (head[6] & 0x7F) << 21 | (head[7] & 0x7F) << 14 | (head[8] & 0x7F) << 7 | (head[9] & 0x7F)
-    return 10 + size + (10 if head[5] & 0x10 else 0)
-
-
-def is_flac(path):
-    """True when the file starts with the FLAC marker, or with an ID3v2 tag and then the marker (False when it cannot
-    be read: the WAV reader reports that)."""
-    try:
-        f = open(path, 'rb')
-    except OSError:
-        return False
-    with f:
-        head = f.read(10)
-        if head[0:4] == FLAC_MAGIC:
-            return True
-        skip = id3v2_size(head)
-        if not skip:
-            return False
-        f.seek(skip)
-        return f.read(4) == FLAC_MAGIC
-
-
-class FlacFile(object):
-    """FLAC metadata reader: an optional leading ID3v2 tag, the marker, then the metadata blocks.  STREAMINFO (which
-    must come first) gives the stream parameters; every other block (PADDING, APPLICATION, SEEKTABLE, VORBIS_COMMENT,
-    CUESHEET, PICTURE) is skipped.  `frame_offset` is where the first audio frame starts; the frames are decoded on the
-    GPU (sb_flac_decode_file / sb_flac_decode_frames)."""
-
-    def __init__(self, path):
-        with open(path, 'rb') as f:
-            self.data = f.read()
-        self._parse(self.data, path)
-
-    @classmethod
-    def from_bytes(cls, data, name):
-        """The metadata of `data` (a Matroska track's CodecPrivate: the marker and the metadata blocks, no frames);
-        messages name `name`."""
-        self = object.__new__(cls)
-        self.data = bytes(data)
-        self._parse(self.data, name)
-        return self
-
-    def _parse(self, d, path):
-        at = id3v2_size(d[:10])
-        if d[at:at + 4] != FLAC_MAGIC:
-            raise SushiError('{0}: not a FLAC file'.format(path))
-        at += 4
-        self.blocks = []
-        have_info = False
-        while True:
-            if at + 4 > len(d):
-                raise SushiError('{0}: FLAC metadata block header at byte {1} is truncated'.format(path, at))
-            last, kind = d[at] >> 7, d[at] & 0x7F
-            size = int.from_bytes(d[at + 1:at + 4], 'big')
-            body = d[at + 4:at + 4 + size]
-            if len(body) < size or kind == 127:
-                raise SushiError('{0}: invalid FLAC metadata block at byte {1}'.format(path, at))
-            if (kind == 0) != (not self.blocks):
-                raise SushiError('{0}: STREAMINFO must be the first and only STREAMINFO metadata block'.format(path))
-            if kind == 0:
-                if size < 34:
-                    raise SushiError('{0}: STREAMINFO of {1} bytes'.format(path, size))
-                self.min_block, self.max_block = struct.unpack('>HH', body[0:4])
-                packed = int.from_bytes(body[10:18], 'big')
-                self.framerate = packed >> 44
-                self.channels_count = ((packed >> 41) & 7) + 1
-                self.bits_per_sample = ((packed >> 36) & 31) + 1
-                self.total_samples = packed & ((1 << 36) - 1)
-                have_info = True
-            self.blocks.append(FLAC_BLOCK_NAMES.get(kind, 'reserved {0}'.format(kind)))
-            at += 4 + size
-            if last:
-                break
-        if not have_info:
-            raise SushiError('{0}: FLAC file without STREAMINFO'.format(path))
-        if self.framerate < 1:
-            raise SushiError('{0}: FLAC STREAMINFO sample rate is 0'.format(path))
-        self.frame_offset = at
-
-    def check_depth(self):
-        """SushiError unless the samples have 16 or 24 bits, the depths the GPU decoder takes."""
-        if self.bits_per_sample not in (16, 24):
-            raise SushiError('FLAC with {0} bits per sample is not supported (16 or 24)'.format(self.bits_per_sample))
-
-
-_CODEC_NAMES = {'flac': 'FLAC', 'alac': 'ALAC', 'truehd': 'TrueHD', 'pcm_bluray': 'BD-LPCM', 'wavpack': 'WavPack', 'tta': 'TTA'}
-
-
-def _refuse_host(path, codec, loader):
-    """Compressed inputs are decoded on the GPU only."""
-    if loader != 'gpu':
-        raise SushiError("{0}: {1} input needs loader='gpu' (there is no host {1} decoder)".format(path, codec))
-
-
-def _decode(lib, name, *args):
-    """The sb_pcm handle a decoder entry point returns through its last argument."""
-    h = ctypes.c_void_p()
-    with nvtx_range('sushi_b200: ' + name):
-        _native.check(getattr(lib, name)(*args, ctypes.byref(h)), name)
-    return h
-
-
-def _decode_frames(lib, name, data, offsets, blocks, *args):
-    """_decode of frames listed in `data`: frame f starts at offsets[f]; blocks[f] is the file offset errors name."""
-    buf = np.frombuffer(data + b'\0', dtype=np.uint8)          # never empty
-    offsets = np.ascontiguousarray(offsets, np.int64)
-    blocks = np.ascontiguousarray(blocks, np.int64)
-    return _decode(lib, name, buf.ctypes.data_as(ctypes.c_void_p), len(data) or 1, offsets.ctypes.data_as(_native.c_i64p),
-                   blocks.ctypes.data_as(_native.c_i64p), len(offsets), *args)
-
-
-def _decode_blocks(lib, data, table, stream):
-    """_decode of sb_wavpack_decode_blocks on the blocks of `table` (wavpack's 8-column block table) in `data`"""
-    buf = np.frombuffer(data, dtype=np.uint8)
-    table = np.ascontiguousarray(table, np.int64)
-    return _decode(lib, 'sb_wavpack_decode_blocks', buf.ctypes.data_as(ctypes.c_void_p), len(data),
-                   table.ctypes.data_as(_native.c_i64p), len(table), stream.channels, stream.rate)
-
-
-def decode_downmix(raw, sample_width, channels):
-    """bytes -> float32 mono; int24 keeps the top 16 bits (wav.py:68-74); channels are
-    summed left to right in float32, then divided (wav.py:88-90)."""
-    if sample_width == 2:
-        pcm = np.frombuffer(raw, dtype='<i2', count=len(raw) // 2)
-    elif sample_width == 3:
-        b = np.frombuffer(raw, dtype=np.uint8, count=(len(raw) // 3) * 3).reshape(-1, 3)
-        pcm = (b[:, 1].astype(np.uint16) | (b[:, 2].astype(np.uint16) << 8)).view(np.int16)
-    else:
-        raise SushiError('Unsupported sample width: {0}'.format(sample_width))
-    samples = pcm.astype(np.float32)
-    if channels == 1:
-        return samples
-    frames = len(samples) // channels
-    if frames * channels != len(samples):
-        logging.error("Length of audio channels didn't match. This might result in broken output")
-    acc = samples[0::channels][:frames].copy()
-    for ch in range(1, channels):
-        acc += samples[ch::channels][:frames]
-    acc /= np.float32(channels)
-    return acc
-
-
-def nearest_index_map(n_in, n_out):
-    """Source index of every output sample of cv2.resize(..., INTER_NEAREST) on a
-    (1, n_in) row resized to (1, n_out): floor(x * (1 / (n_out / n_in))) in fp64,
-    clamped to n_in-1 (OpenCV resizeNN; pinned against cv2 in tests)."""
-    inv = 1.0 / (float(n_out) / float(n_in))
-    idx = np.floor(np.arange(n_out, dtype=np.float64) * inv).astype(np.int64)
-    np.minimum(idx, n_in - 1, out=idx)
-    return idx
-
-
-
-
-def normalise_host(data, sample_type):
-    """Median-clip normalisation of a padded float32 (1,N) array, in place semantics of
-    wav.py:145-156 (float32 arithmetic throughout, medians over the padded array)."""
-    flat = data.reshape(-1)
-    max_value = np.float32(np.median(flat[flat >= 0])) * np.float32(3)
-    min_value = np.float32(np.median(flat[flat <= 0])) * np.float32(3)
-    np.clip(data, min_value, max_value, out=data)
-    data -= min_value
-    data /= (max_value - min_value)
-    if sample_type == 'uint8':
-        data *= np.float32(255.0)
-        data += np.float32(0.5)
-        data = data.astype(np.uint8)
-    return data, float(min_value), float(max_value)
 
 
 class StreamGeometry(object):
@@ -364,221 +99,50 @@ class WavStream(StreamGeometry):
     def __init__(self, path, sample_rate=12000, sample_type='uint8', device=None, loader='gpu', track=None):
         """loader='gpu' (default): decode / resample / pad / normalise on the GPU (sb_load_pcm +
         sb_normalise); loader='host' runs the NumPy mirror of the same arithmetic and uploads the
-        result (kept as the cross-check; both give bit-identical .data).  A Matroska file loads its audio track
-        `track` (a stream id; None: the only audio track, else the default one, as the reference selects); `path` may
-        also be an opened MatroskaFile, whose frames then come from one walk shared with the script and timecodes.  A
-        transport stream (.m2ts, .mts, .m2t, .ts, or an opened TransportStream) loads its audio stream `track` the
-        same way, and so does an MP4 / QuickTime file (.mp4, .m4a, .m4v, .mov, or an opened Mp4File)."""
+        result (kept as the cross-check; both give bit-identical .data).  `path` is a file of any format in
+        inputs.FORMATS, or an opened MatroskaFile, Mp4File or TransportStream (left open; a MatroskaFile's frames then
+        come from one walk shared with the script and timecodes).  A container loads its audio stream `track` (a stream
+        id; None: the only audio track, else the default one, as the reference selects)."""
         if sample_type not in _DTYPES:
             raise SushiError('Unknown sample type of WAV stream, must be uint8 or float32')
         self._handle = None
         before_read = time()
-        if isinstance(path, mpegts.TransportStream) or mpegts.is_transport_stream(path):
-            name, load = 'transport stream', self._load_ts
-        elif isinstance(path, mp4.Mp4File) or (not isinstance(path, matroska.MatroskaFile) and mp4.is_mp4(path)):
-            name, load = 'MP4', self._load_mp4
-        elif isinstance(path, matroska.MatroskaFile) or matroska.is_matroska(path):
-            name, load = 'Matroska', self._load_matroska
-        elif truehd.is_truehd(path):
-            name, load = 'TrueHD', self._load_truehd
-        elif wavpack.is_wavpack(path):
-            name, load = 'WavPack', self._load_wavpack
-        elif tta.is_tta(path):
-            name, load = 'TTA', self._load_tta
-        elif is_flac(path):
-            name, load = 'FLAC', self._load_flac
-        else:
-            name, load = 'WAV', self._load_wav
-        load(path, sample_rate, sample_type, device, loader, track)
+        reader, name = open_input(path)
+        try:
+            audio = reader.select_audio(track)
+            if audio.label is None:
+                self._load_pcm(audio.pcm, sample_rate, sample_type, device, loader)
+            else:
+                # compressed inputs are decoded on the GPU only
+                if loader != 'gpu':
+                    raise SushiError("{0}: {1} input needs loader='gpu' (there is no host {1} decoder)".format(
+                        audio.path, audio.label))
+                self._load_decoded(audio.decode(device), sample_rate, sample_type, device, audio.check)
+        except Exception as e:
+            if isinstance(e, SushiError) or name != 'WAV':
+                raise
+            raise SushiError('Error while loading {0}: {1}'.format(path, e))        # as the reference does (wav.py:158-159)
+        finally:
+            if reader is not path and hasattr(reader, 'close'):
+                reader.close()
         logging.info('Done reading {0} {1} in {2}s'.format(name, path, time() - before_read))
 
-    def _load_wav(self, path, sample_rate, sample_type, device, loader, track):
-        stream = DownmixedWavFile(path)
-        try:
-            if loader == 'gpu':
-                # what the reference's chunk loop reads (wav.py:125-137): whole seconds from the start of the data
-                # chunk, so the last read can run past the chunk or stop short at the end of a truncated file
-                reads = math.ceil(stream.frames_count / float(stream.framerate))
-                pcm = stream.read_raw(reads * stream.framerate)
-                self._load_gpu(pcm, stream.frames_count, stream.channels_count, stream.sample_width,
-                               stream.framerate, sample_rate, sample_type, device)
-            else:
-                self._load(stream, sample_rate, sample_type)
-                self._upload(device)
-        except SushiError:
-            raise
-        except Exception as e:
-            raise SushiError('Error while loading {0}: {1}'.format(path, e))
-        finally:
-            stream.close()
-
-    def _load_flac(self, path, sample_rate, sample_type, device, loader, track):
-        """A FLAC file: its frames are found by their sync codes and decoded on the GPU (sb_flac_decode_file)."""
-        flac = FlacFile(path)
-        flac.check_depth()
-        _refuse_host(path, 'FLAC', loader)
-        lib = _native.lib(device)
-        buf = np.frombuffer(flac.data, dtype=np.uint8)
-        h = _decode(lib, 'sb_flac_decode_file', buf.ctypes.data_as(ctypes.c_void_p), len(flac.data), flac.frame_offset,
-                    flac.channels_count, flac.bits_per_sample, flac.framerate)
-
-        def check(frames):
-            # after the frames passed their checks, which name a damaged frame more precisely than the total does
-            if flac.total_samples and flac.total_samples != frames:
-                raise SushiError('{0}: FLAC STREAMINFO says {1} samples, the frames hold {2}'.format(
-                    path, flac.total_samples, frames))
-        self._load_decoded(h, sample_rate, sample_type, device, check)
-
-    def _load_truehd(self, path, sample_rate, sample_type, device, loader, track):
-        """A raw TrueHD stream: one block holding every access unit (sb_truehd_decode)."""
-        data, _ = truehd.read_stream(path)
-        _refuse_host(path, 'TrueHD', loader)
-        # one block; a negative file offset makes messages name each access unit's own offset
-        h = _decode_frames(_native.lib(device), 'sb_truehd_decode', data, np.zeros(1, np.int64), np.full(1, -1, np.int64))
-        self._load_decoded(h, sample_rate, sample_type, device)
-
-    def _load_wavpack(self, path, sample_rate, sample_type, device, loader, track):
-        """A raw WavPack (.wv) file: its block chain walked on the host (wavpack.WavPackFile, which refuses what cannot
-        be decoded and a broken chain), every block decoded on the GPU (sb_wavpack_decode_blocks)."""
-        f = wavpack.WavPackFile(path)
-        _refuse_host(path, 'WavPack', loader)
-        self._load_decoded(_decode_blocks(_native.lib(device), f.data, f.table, f.stream), sample_rate, sample_type,
-                           device)
-
-    def _load_tta(self, path, sample_rate, sample_type, device, loader, track):
-        """A raw TTA (.tta) file: its header and seek table read on the host (tta.TTAFile, which refuses what cannot be
-        decoded and damage they show), every frame decoded on the GPU (sb_tta_decode_frames)."""
-        f = tta.TTAFile(path)
-        _refuse_host(path, 'TTA', loader)
-        # the file's bytes as read, up to the end of the audio: frames at their file offsets, no copy
-        buf = np.frombuffer(f.data, dtype=np.uint8)
-        h = _decode(_native.lib(device), 'sb_tta_decode_frames', buf.ctypes.data_as(ctypes.c_void_p), f.end,
-                    f.where.ctypes.data_as(_native.c_i64p), f.where.ctypes.data_as(_native.c_i64p), len(f.where),
-                    f.config.ctypes.data_as(_native.c_i32p))
-        self._load_decoded(h, sample_rate, sample_type, device)
-
-    def _load_ts(self, path, sample_rate, sample_type, device, loader, track):
-        """A transport stream's BD-LPCM or TrueHD stream (sb_ts_*).  The file is read in chunks of mpegts.CHUNK_BYTES
-        into two page-locked buffers, one after the other, so that the GPU scans one chunk while the next is read."""
-        ts = path if isinstance(path, mpegts.TransportStream) else mpegts.TransportStream(path)
-        s = ts.select('audio', track)
-        kind = mpegts.audio_codec(s)
-        _refuse_host(ts.path, _CODEC_NAMES[kind], loader)
-        lib = _native.lib(device)
-        t = ctypes.c_void_p()
-        codec = _native.SB_TS_TRUEHD if kind == 'truehd' else _native.SB_TS_PCM_BLURAY
-        _native.check(lib.sb_ts_open(ts.packet_size, s.pid, codec, ctypes.byref(t)), 'sb_ts_open')
-        cut = ctypes.c_int32()
-        try:
-            size = max(ts.packet_size, mpegts.CHUNK_BYTES // ts.packet_size * ts.packet_size)
-            buffers = [_native.pinned_empty((size,), np.uint8) for _ in range(2)]
-            with nvtx_range('sushi_b200: sb_ts_feed'):
-                for view, pos in ts.chunks(buffers):
-                    arr = np.frombuffer(view, np.uint8)
-                    _native.check(lib.sb_ts_feed(t, arr.ctypes.data_as(ctypes.c_void_p), len(arr), pos), 'sb_ts_feed')
-            del buffers
-            h = _decode(lib, 'sb_ts_finish', t, ctypes.byref(cut))
-        finally:
-            lib.sb_ts_destroy(t)
-        if cut.value:
-            logging.warning('{0}: the last PES packet of stream {1} is cut short; its whole sample frames are '
-                            'kept'.format(ts.path, s.id))
-        self._load_decoded(h, sample_rate, sample_type, device)
-
-    def _load_matroska(self, path, sample_rate, sample_type, device, loader, track):
-        """A Matroska audio track (_load_track; a FLAC track's frame numbers and stale STREAMINFO total are not
-        checked).  `path` is a file name or an opened MatroskaFile (left open; the track's table is released from
-        it)."""
-        opened = isinstance(path, matroska.MatroskaFile)
-        mkv = path if opened else matroska.MatroskaFile(path)
-        try:
-            t = mkv.select('audio', track)
-            kind = matroska.audio_codec(t)
-
-            def read_frames():
-                table = mkv.frames([t.id])[t.id]
-                mkv.release([t.id])
-                return table
-            pcm = (t.channels, int(t.sampling_frequency), t.bit_depth // 8, False) if kind == 'pcm' else None
-            # WavPack: the stream version, and the channel count a multi-block frame must code
-            config = (t.codec_private, t.channels) if kind == 'wavpack' else t.codec_private
-            if kind == 'tta':
-                # the decoder config FFmpeg builds from the track and the Segment's Duration
-                config = tta.matroska_config(t, mkv.timestamp_scale, mkv.duration)
-            self._load_track(mkv.path, t.id, kind, config, pcm, read_frames, sample_rate, sample_type, device,
-                             loader)
-        finally:
-            if not opened:
-                mkv.close()
-
-    def _load_mp4(self, path, sample_rate, sample_type, device, loader, track):
-        """An MP4 / QuickTime audio track (_load_track).  `path` is a file name or an opened Mp4File (left open)."""
-        opened = isinstance(path, mp4.Mp4File)
-        f = path if opened else mp4.Mp4File(path)
-        try:
-            t = f.select('audio', track)
-            kind = mp4.audio_codec(t)
-            f.check_edits(t)
-            pcm = (t.channels, t.rate) + mp4.PCM_DECODED[t.codec] if kind == 'pcm' else None
-            self._load_track(f.path, t.id, kind, t.config, pcm, lambda: f.frames(t), sample_rate, sample_type, device,
-                             loader)
-        finally:
-            if not opened:
-                f.close()
-
-    def _load_track(self, path, track_id, kind, config, pcm, read_frames, sample_rate, sample_type, device, loader):
-        """A container's audio track loads exactly as the plain PCM WAV of the samples FFmpeg's decoder returns, frames
-        concatenated in container order (timestamp gaps are not filled).  `kind` is 'flac', 'alac', 'truehd', 'wavpack',
-        'tta' or 'pcm'; `config` the codec's configuration (FLAC metadata blocks, the ALACSpecificConfig, WavPack's
-        (CodecPrivate, channel count), TTA's decoder config); `pcm` (channels, rate, sample width, big-endian) for PCM.  read_frames() reads
-        the track's FrameTable, only once every refusal has passed.  FLAC, ALAC, WavPack, TTA and TrueHD frames are
-        decoded on the GPU where the table puts them, errors naming the file offset of a frame's block; PCM goes through sb_load_pcm (little-endian), sb_pcm_from_be (big-endian) or, for
-        loader='host', the host loader."""
-        name = '{0} track {1}'.format(path, track_id)
-        if kind == 'flac':
-            info = FlacFile.from_bytes(config, name)
-            info.check_depth()
-        if kind != 'pcm':
-            _refuse_host(path, _CODEC_NAMES[kind], loader)
-        table = read_frames()
-        if kind == 'pcm':
-            channels, rate, width, big = pcm
-            frames = len(table.data) // (channels * width)
-            data = table.data[:frames * channels * width]
-            if loader != 'gpu':
-                if big:
-                    data = np.frombuffer(data, np.uint8).reshape(-1, width)[:, ::-1].tobytes()
-                self._load(DownmixedWavFile.from_bytes(data, channels, rate, width), sample_rate, sample_type)
-                self._upload(device)
-            elif big:
-                buf = np.frombuffer(data, dtype=np.uint8)
-                h = _decode(_native.lib(device), 'sb_pcm_from_be', buf.ctypes.data_as(ctypes.c_void_p), frames, channels,
-                            width, rate)
-                self._load_decoded(h, sample_rate, sample_type, device)
-            else:
-                self._load_gpu(data, frames, channels, width, rate, sample_rate, sample_type, device)
-            return
-        table.refuse_empty(path, _CODEC_NAMES[kind])
-        if kind == 'wavpack':
-            blocks, stream = wavpack.matroska_table(table, config[0], track_id, config[1])
-        lib = _native.lib(device)
-        if kind == 'flac':
-            h = _decode_frames(lib, 'sb_flac_decode_frames', table.data, table.offset, table.block, info.channels_count,
-                               info.bits_per_sample, info.framerate)
-        elif kind == 'wavpack':
-            h = _decode_blocks(lib, table.data, blocks, stream)
-        elif kind == 'tta':
-            h = _decode_frames(lib, 'sb_tta_decode_frames', table.data, table.offset, table.block,
-                               config.ctypes.data_as(_native.c_i32p))
-        elif kind == 'alac':
-            fl, _, depth, pb, mb, kb, channels, _, _, _, rate = struct.unpack('>IBBBBBBHIII', config[:24])
-            cfg = np.array([fl, depth, pb, mb, kb, channels, rate], np.int32)
-            h = _decode_frames(lib, 'sb_alac_decode_frames', table.data, table.offset, table.block,
-                               cfg.ctypes.data_as(_native.c_i32p))
+    def _load_pcm(self, pcm, sample_rate, sample_type, device, loader):
+        """Integer PCM as a reader lays it out, pcm() -> (bytes, frames, channels, sample width, rate, big-endian):
+        sb_load_pcm (little-endian), sb_pcm_from_be (big-endian) or, for loader='host', the host loader."""
+        data, frames, channels, width, rate, big = pcm()
+        if loader != 'gpu':
+            if big:
+                data = np.frombuffer(data, np.uint8).reshape(-1, width)[:, ::-1].tobytes()
+            self._load(DownmixedWavFile.from_bytes(data, channels, rate, width, frames), sample_rate, sample_type)
+            self._upload(device)
+        elif big:
+            buf = np.frombuffer(data, dtype=np.uint8)
+            h = _native.decode(device, 'sb_pcm_from_be', buf.ctypes.data_as(ctypes.c_void_p), frames, channels, width,
+                               rate)
+            self._load_decoded(h, sample_rate, sample_type, device)
         else:
-            truehd.MajorSync(table.data[:64], name)
-            h = _decode_frames(lib, 'sb_truehd_decode', table.data, table.offset, table.block)
-        self._load_decoded(h, sample_rate, sample_type, device)
+            self._load_gpu(data, frames, channels, width, rate, sample_rate, sample_type, device)
 
     def _load_decoded(self, h, sample_rate, sample_type, device, check=None):
         """_load_gpu_with on a decoder's sb_pcm handle `h` (sb_pcm_load), which it destroys; check(frames) may refuse
@@ -864,16 +428,6 @@ class WavStream(StreamGeometry):
         return [(np.float32(diff[q]), t0[q] + (int(idx[q]) / rate)) for q in range(len(plan))]
 
     # -- batched surface (what the sharded benchmark and the batched shift solver use) ------
-    @staticmethod
-    def _template_ranges(src_stream, starts, ends):
-        """(offset, length) of get_substream(starts[q], ends[q]) on src_stream, NumPy slice clamping included."""
-        total = src_stream.total_samples
-        lo = np.trunc(src_stream.sample_rate * np.asarray(starts, np.float64)).astype(np.int64) + src_stream.padding_size
-        hi = np.trunc(src_stream.sample_rate * np.asarray(ends, np.float64)).astype(np.int64) + src_stream.padding_size
-        lo = np.where(lo < 0, np.maximum(lo + total, 0), np.minimum(lo, total))
-        hi = np.where(hi < 0, np.maximum(hi + total, 0), np.minimum(hi, total))
-        return lo, np.maximum(hi - lo, 0)
-
     def find_substream_batch(self, src_stream, starts, ends, centers, windows):
         """Batched find_substream: returns (diffs float32[count], times float64[count])."""
         with nvtx_range('sushi_b200: find_substream_batch'):
@@ -926,7 +480,7 @@ class WavStream(StreamGeometry):
         # over the next 48 groups
         if cache:
             total, pad, rate = src_stream.total_samples, src_stream.padding_size, src_stream.sample_rate
-            lo = int(rate * float(groups[idx][0].start)) + pad          # trunc toward zero, like _template_ranges
+            lo = int(rate * float(groups[idx][0].start)) + pad          # trunc toward zero, like plan_queries
             hi = int(rate * float(groups[idx][-1].end)) + pad
             lo = max(lo + total, 0) if lo < 0 else min(lo, total)
             hi = max(hi + total, 0) if hi < 0 else min(hi, total)
