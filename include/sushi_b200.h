@@ -39,7 +39,7 @@
 extern "C" {
 #endif
 
-#define SB_ABI_VERSION 11
+#define SB_ABI_VERSION 12
 
 /* status codes */
 #define SB_OK            0
@@ -242,6 +242,19 @@ int sb_pcm_destroy(sb_pcm* pcm);
 /* Big-endian 16- or 24-bit interleaved PCM (QuickTime `twos` / `in24`, ISO `ipcm`): loaded through sb_pcm_load it
  * gives bit for bit what sb_load_pcm gives on the byte-swapped data. */
 int sb_pcm_from_be(const void* pcm_host, int64_t frames, int channels, int sample_width, int framerate, sb_pcm** out);
+
+/* Little-endian 16- or 24-bit interleaved PCM (ABI version 12; Matroska `A_PCM/INT/LIT`, MP4 `sowt` / `lpcm`): the
+ * top 16 bits of each sample, as sb_load_pcm reads them. */
+int sb_pcm_from_le(const void* pcm_host, int64_t frames, int channels, int sample_width, int framerate, sb_pcm** out);
+
+/* The ffmpeg command line's `-ac 1 -ar <out_rate> -acodec pcm_s16le` on S16 audio (ABI version 12): a new mono
+ * handle at out_rate holding what libswresample 6.1.100 with its default options gives on its x86-64 FMA3 path, bit
+ * for bit and frame for frame.  `layout` is FFmpeg's channel mask of the input (AV_CH_*; its bit count is the
+ * handle's channel count).  Equal rates take the integer Q15 downmix and a mono input is copied; otherwise every
+ * channel is resampled in float by the Kaiser-windowed polyphase filter and then remixed.  Fails on a layout
+ * libswresample refuses or with channels other than FL FR FC LFE BL BR FLC FRC BC SL SR, and on a rate pair whose
+ * filter window exceeds 48 KB of shared memory per 32 outputs.  `in` is left as it is. */
+int sb_pcm_swr(const sb_pcm* in, uint64_t layout, int out_rate, sb_pcm** out);
 
 /* FLAC (ABI version 3).  16 and 24 bits per sample and 1 to 8 channels are accepted; the caller has read STREAMINFO
  * and passes its channel count, bits per sample and sample rate.  Every frame must decode, pass its CRC-16 and end

@@ -17,7 +17,7 @@ LIB_PATH = os.path.join(_HERE, 'libsushi_b200.so')
 
 SB_OK = 0
 SB_U8, SB_F32 = 0, 1
-ABI_VERSION = 11
+ABI_VERSION = 12
 SB_TS_PCM_BLURAY, SB_TS_TRUEHD = 0, 1
 
 c_i64 = ctypes.c_int64
@@ -73,6 +73,8 @@ PROTOTYPES = {
     'sb_pcm_load': (ctypes.c_int, [c_vp, ctypes.c_int, c_i64, c_i64, ctypes.POINTER(c_vp)]),
     'sb_pcm_destroy': (ctypes.c_int, [c_vp]),
     'sb_pcm_from_be': (ctypes.c_int, [c_vp, c_i64, ctypes.c_int, ctypes.c_int, ctypes.c_int, ctypes.POINTER(c_vp)]),
+    'sb_pcm_from_le': (ctypes.c_int, [c_vp, c_i64, ctypes.c_int, ctypes.c_int, ctypes.c_int, ctypes.POINTER(c_vp)]),
+    'sb_pcm_swr': (ctypes.c_int, [c_vp, ctypes.c_uint64, ctypes.c_int, ctypes.POINTER(c_vp)]),
     'sb_flac_decode_file': (ctypes.c_int, [c_vp, c_i64, c_i64, ctypes.c_int, ctypes.c_int, ctypes.c_int,
                                            ctypes.POINTER(c_vp)]),
     'sb_flac_decode_frames': (ctypes.c_int, [c_vp, c_i64, c_i64p, c_i64p, c_i64, ctypes.c_int, ctypes.c_int, ctypes.c_int,

@@ -7,6 +7,11 @@ import numpy as np
 from . import _native
 
 
+def bit_depth(config):
+    """The bit depth of an ALACSpecificConfig."""
+    return struct.unpack('>IBB', config[:6])[2]
+
+
 def track_decoder(config):
     """decode(device, table) of an ALAC track (sb_alac_decode_frames on its FrameTable).  `config` is the 24-byte
     ALACSpecificConfig: frame length, bit depth, pb, mb, kb, channels and sample rate reach the decoder."""

@@ -15,7 +15,7 @@ import os
 import sys
 import time
 
-from . import __version__
+from . import __version__, swr
 from .common import SushiError
 from .inputs import FORMATS
 from .pipeline import shift_script
@@ -74,6 +74,9 @@ def create_arg_parser():
                         help=argparse.SUPPRESS)
     parser.add_argument('--sample-rate', default=12000, type=int, metavar='<rate>', dest='sample_rate',
                         help='Downsampled audio sample rate. [%(default)s]')
+    parser.add_argument('--ffmpeg-audio', action='store_true', dest='ffmpeg_audio',
+                        help='Load inputs other than WAV files as the reference\'s ffmpeg call writes them: '
+                             'libswresample\'s downmix and resample of 16-bit sources, bit for bit')
 
     # stream indices select streams of a Matroska input; WAV and FLAC inputs have one of each, so they are ignored
     parser.add_argument('--src-audio', default=None, type=int, metavar='<id>', dest='src_audio_idx',
@@ -138,9 +141,15 @@ def _open_input(path):
         raise SushiError('{0} (it does not open as {1}: {2})'.format(refusal, fmt.opens_as, e))
 
 
-def _select_audio(reader, idx):
-    """The stream id of a container input's audio track (None for the other inputs), refusing what cannot be decoded."""
-    return None if reader is None else reader.select_audio(idx).id
+def _select_audio(reader, idx, ffmpeg_audio=False):
+    """The stream id of a container input's audio track (None for the other inputs), refusing what cannot be decoded
+    and, with --ffmpeg-audio, what FFmpeg decodes to S32."""
+    if reader is None:
+        return None
+    audio = reader.select_audio(idx)
+    if ffmpeg_audio:
+        swr.check(audio)
+    return audio.id
 
 
 def run(args):
@@ -185,8 +194,8 @@ def run(args):
 
 
 def _run(args, ignore_chapters, src_mkv, dst_mkv, written):
-    src_track = _select_audio(src_mkv, args.src_audio_idx)
-    dst_track = _select_audio(dst_mkv, args.dst_audio_idx)
+    src_track = _select_audio(src_mkv, args.src_audio_idx, args.ffmpeg_audio)
+    dst_track = _select_audio(dst_mkv, args.dst_audio_idx, args.ffmpeg_audio)
     # files taken out of the inputs, written once every check has passed: (path, function giving the text); and per
     # Matroska input, the tracks one walk over its clusters reads: (frames read, block times only)
     extract = []
@@ -288,6 +297,8 @@ def _run(args, ignore_chapters, src_mkv, dst_mkv, written):
                                         src_timecodes_file, dst_timecodes_file)
 
     tracks = {} if src_track is None and dst_track is None else dict(src_track=src_track, dst_track=dst_track)
+    if args.ffmpeg_audio:
+        tracks['ffmpeg_audio'] = True
     src = args.source if src_mkv is None else src_mkv
     dst = args.destination if dst_mkv is None else dst_mkv
     return shift_script(src, dst, src_script_path, dst_script_path,

@@ -13,8 +13,11 @@ class SushiError(Exception):
 # loads.  `label` names a codec the GPU decodes ('FLAC', 'TrueHD', 'BD-LPCM', ...) and is None for PCM; `id` is the
 # stream id in a container; `path` names the file in messages.  A codec has decode(device) -> the sb_pcm handle of the
 # decoded samples (it loads the library, and reads a container track's frames first) and may have check(frames), which
-# refuses the decoded frame count; PCM has pcm() -> (bytes, frames, channels, sample width, rate, big-endian).
-Audio = collections.namedtuple('Audio', 'label id path decode pcm check', defaults=(None,) * 5)
+# refuses the decoded frame count; PCM has pcm() -> (bytes, frames, channels, sample width, rate, big-endian).  For the
+# --ffmpeg-audio conversion (sushi_b200/swr.py) a reader also tells what FFmpeg's decoder outputs: `fmt` its sample
+# format ('S16' or 'S32'; None when the reader cannot tell before decoding), `bits` the source's bit depth, and
+# `layout` its channel mask (AV_CH_* bits) by channel count.
+Audio = collections.namedtuple('Audio', 'label id path decode pcm check fmt bits layout', defaults=(None,) * 8)
 
 
 def clip(value, minimum, maximum):

@@ -2,7 +2,8 @@
 //   K1  sb_load_pcm   int16/int24 decode, channel average, per-chunk nearest-neighbour resample
 //                     (cv2.resize INTER_NEAREST index map), edge padding      wav.py:64-91,125-141
 //   K2  sb_normalise  3 x median clip, rescale to [0,1], optional uint8 quantisation  wav.py:145-156
-// sb_pcm_load runs K1 on a decoder's int16 PCM (an sb_pcm); sb_pcm_from_be makes one from big-endian PCM (k_pcm_be).
+// sb_pcm_load runs K1 on a decoder's int16 PCM (an sb_pcm); sb_pcm_from_be / sb_pcm_from_le make one from big- or
+// little-endian PCM (k_pcm_be, k_pcm_le).
 // Everything is float32 with explicitly rounded operations (no FMA contraction), in the order the
 // reference applies them, so the result is bit-identical to the NumPy/OpenCV loader.
 #include "sb_internal.h"
@@ -340,6 +341,43 @@ k_pcm_be(const uint8_t* __restrict__ in, int64_t n, int width, int16_t* __restri
     }
 }
 
+// little-endian 16- or 24-bit samples -> the top 16 bits as int16
+__global__ void __launch_bounds__(256)
+k_pcm_le(const uint8_t* __restrict__ in, int64_t n, int width, int16_t* __restrict__ out) {
+    for (int64_t i = (int64_t)blockIdx.x * blockDim.x + threadIdx.x; i < n; i += (int64_t)gridDim.x * blockDim.x) {
+        const uint8_t* p = in + i * width + (width - 2);
+        out[i] = (int16_t)(uint16_t)(p[0] | ((unsigned)p[1] << 8));
+    }
+}
+
+// sb_pcm_from_be / sb_pcm_from_le: upload, one conversion kernel, hand the int16 PCM over
+int pcm_from_bytes(const void* pcm_host, int64_t frames, int channels, int sample_width, int framerate, bool big,
+                   sb_pcm** out, const char* who) {
+    Ctx& c = ctx();
+    if (!c.inited) SB_FAIL(SB_ESTATE, "%s: library not initialised (call sb_init)", who);
+    if (!pcm_host || !out) SB_FAIL(SB_EINVAL, "%s: NULL argument", who);
+    if (sample_width != 2 && sample_width != 3) SB_FAIL(SB_EINVAL, "Unsupported sample width: %d", sample_width);
+    if (frames < 0 || channels < 1) SB_FAIL(SB_EINVAL, "%s: bad geometry", who);
+    const int64_t n = frames * channels;
+    unsigned char* d_in = nullptr;
+    int16_t* d_pcm = nullptr;
+    int rc = pool_alloc((void**)&d_in, (size_t)n * sample_width + 16);
+    if (rc == SB_OK) rc = pool_alloc((void**)&d_pcm, sizeof(int16_t) * (size_t)n + 16);
+    if (rc != SB_OK) { pool_free(d_in); pool_free(d_pcm); return rc; }
+    cudaError_t e = cudaMemcpyAsync(d_in, pcm_host, (size_t)n * sample_width, cudaMemcpyHostToDevice, c.stream);
+    if (e == cudaSuccess && n > 0) {
+        ProfScope ps(big ? "pcm_be" : "pcm_le");
+        const int grid = (int)std::max<int64_t>(1, std::min<int64_t>((n + 255) / 256, (int64_t)c.sm_count * 16));
+        if (big) k_pcm_be<<<grid, 256, 0, c.stream>>>(d_in, n, sample_width, d_pcm);
+        else k_pcm_le<<<grid, 256, 0, c.stream>>>(d_in, n, sample_width, d_pcm);
+        e = cudaGetLastError();
+    }
+    if (e == cudaSuccess) e = cudaStreamSynchronize(c.stream);             // pcm_host may be reused by the caller
+    pool_free(d_in);
+    if (e != cudaSuccess) { pool_free(d_pcm); SB_FAIL(SB_ECUDA, "%s: %s", who, cudaGetErrorString(e)); }
+    return pcm_handle(d_pcm, frames, channels, framerate, out);
+}
+
 }  // namespace
 
 namespace sb {
@@ -431,28 +469,11 @@ int sb_pcm_destroy(sb_pcm* pcm) {
 }
 
 int sb_pcm_from_be(const void* pcm_host, int64_t frames, int channels, int sample_width, int framerate, sb_pcm** out) {
-    Ctx& c = ctx();
-    if (!c.inited) SB_FAIL(SB_ESTATE, "sb_pcm_from_be: library not initialised (call sb_init)");
-    if (!pcm_host || !out) SB_FAIL(SB_EINVAL, "sb_pcm_from_be: NULL argument");
-    if (sample_width != 2 && sample_width != 3) SB_FAIL(SB_EINVAL, "Unsupported sample width: %d", sample_width);
-    if (frames < 0 || channels < 1) SB_FAIL(SB_EINVAL, "sb_pcm_from_be: bad geometry");
-    const int64_t n = frames * channels;
-    unsigned char* d_in = nullptr;
-    int16_t* d_pcm = nullptr;
-    int rc = pool_alloc((void**)&d_in, (size_t)n * sample_width + 16);
-    if (rc == SB_OK) rc = pool_alloc((void**)&d_pcm, sizeof(int16_t) * (size_t)n + 16);
-    if (rc != SB_OK) { pool_free(d_in); pool_free(d_pcm); return rc; }
-    cudaError_t e = cudaMemcpyAsync(d_in, pcm_host, (size_t)n * sample_width, cudaMemcpyHostToDevice, c.stream);
-    if (e == cudaSuccess && n > 0) {
-        ProfScope ps("pcm_be");
-        const int grid = (int)std::max<int64_t>(1, std::min<int64_t>((n + 255) / 256, (int64_t)c.sm_count * 16));
-        k_pcm_be<<<grid, 256, 0, c.stream>>>(d_in, n, sample_width, d_pcm);
-        e = cudaGetLastError();
-    }
-    if (e == cudaSuccess) e = cudaStreamSynchronize(c.stream);             // pcm_host may be reused by the caller
-    pool_free(d_in);
-    if (e != cudaSuccess) { pool_free(d_pcm); SB_FAIL(SB_ECUDA, "sb_pcm_from_be: %s", cudaGetErrorString(e)); }
-    return pcm_handle(d_pcm, frames, channels, framerate, out);
+    return pcm_from_bytes(pcm_host, frames, channels, sample_width, framerate, true, out, "sb_pcm_from_be");
+}
+
+int sb_pcm_from_le(const void* pcm_host, int64_t frames, int channels, int sample_width, int framerate, sb_pcm** out) {
+    return pcm_from_bytes(pcm_host, frames, channels, sample_width, framerate, false, out, "sb_pcm_from_le");
 }
 
 int sb_normalise(const sb_stream* raw_f32, int dtype, sb_stream** out, float* min3_out, float* max3_out) {

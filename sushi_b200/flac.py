@@ -6,7 +6,7 @@ import struct
 
 import numpy as np
 
-from . import _native
+from . import _native, swr
 from .common import Audio, SushiError
 
 FLAC_MAGIC = b'fLaC'
@@ -112,7 +112,8 @@ class FlacFile(object):
             if self.total_samples and self.total_samples != frames:
                 raise SushiError('{0}: FLAC STREAMINFO says {1} samples, the frames hold {2}'.format(
                     self.path, self.total_samples, frames))
-        return Audio('FLAC', path=self.path, decode=lambda device: decode_file(device, self), check=check)
+        return Audio('FLAC', path=self.path, decode=lambda device: decode_file(device, self), check=check,
+                     **swr.audio_format(self.bits_per_sample, swr.FLAC))
 
 
 def decode_file(device, flac):

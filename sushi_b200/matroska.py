@@ -24,7 +24,7 @@ import zlib
 
 import numpy as np
 
-from . import _native, alac, flac, truehd, tta, wavpack
+from . import _native, alac, flac, swr, truehd, tta, wavpack
 from .common import Audio, SushiError, py2_round, select_stream
 
 MATROSKA_EXTENSIONS = ('.mkv', '.mka', '.mks', '.webm')
@@ -190,7 +190,7 @@ class FrameTable(object):
         return self.data[self.offset[i]:self.offset[i] + self.size[i]]
 
 
-def track_audio(path, track_id, label, read_frames, decode):
+def track_audio(path, track_id, label, read_frames, decode, **fields):
     """The Audio of a container's audio track of the codec `label`: it loads exactly as the plain PCM WAV of the
     samples FFmpeg's decoder returns, frames concatenated in container order (timestamp gaps are not filled).  The
     order of what can refuse it: the caller has made the track's own refusals (selection, codec, edits, a FLAC track's
@@ -202,7 +202,7 @@ def track_audio(path, track_id, label, read_frames, decode):
         table = read_frames()
         table.refuse_empty(path, label)
         return decode(device, table)
-    return Audio(label, track_id, path, decode=run)
+    return Audio(label, track_id, path, decode=run, **fields)
 
 
 def track_pcm(path, track_id, read_frames, channels, rate, width, big_endian):
@@ -211,7 +211,7 @@ def track_pcm(path, track_id, read_frames, channels, rate, width, big_endian):
         data = read_frames().data
         frames = len(data) // (channels * width)
         return data[:frames * channels * width], frames, channels, width, rate, big_endian
-    return Audio(None, track_id, path, pcm=pcm)
+    return Audio(None, track_id, path, pcm=pcm, **swr.audio_format(8 * width, swr.DEFAULT))
 
 
 class _Source(object):
@@ -697,15 +697,19 @@ class MatroskaFile(object):
                              False)
         if kind == 'flac':
             label, decode = 'FLAC', flac.track_decoder(t.codec_private, name)
+            fields = swr.audio_format(flac.FlacFile.from_bytes(t.codec_private, name).bits_per_sample, swr.FLAC)
         elif kind == 'alac':
             label, decode = 'ALAC', alac.track_decoder(t.codec_private)
+            fields = swr.audio_format(alac.bit_depth(t.codec_private), swr.ALAC)
         elif kind == 'wavpack':
             label, decode = 'WavPack', wavpack.track_decoder(t)
+            fields = {}                             # the bit depth is in the blocks, read when the track decodes
         elif kind == 'tta':
             label, decode = 'TTA', tta.track_decoder(t, self.timestamp_scale, self.duration)
+            fields = swr.audio_format(t.bit_depth, swr.TTA)
         else:
-            label, decode = 'TrueHD', decode_truehd
-        return track_audio(self.path, t.id, label, read_frames, decode)
+            label, decode, fields = 'TrueHD', decode_truehd, {'fmt': 'S32'}
+        return track_audio(self.path, t.id, label, read_frames, decode, **fields)
 
     # -- side products ----------------------------------------------------------------------------------------------
     no_timecodes = None                             # video timestamps can be read (timecodes_text)

@@ -26,7 +26,7 @@ import struct
 
 import numpy as np
 
-from . import alac, flac
+from . import alac, flac, swr
 from .common import SushiError, select_stream
 from .matroska import FrameTable, track_audio, track_pcm
 
@@ -494,10 +494,13 @@ class Mp4File(object):
         if kind == 'pcm':
             return track_pcm(self.path, t.id, lambda: self.frames(t), t.channels, t.rate, *PCM_DECODED[t.codec])
         if kind == 'flac':
-            label, decode = 'FLAC', flac.track_decoder(t.config, '{0} track {1}'.format(self.path, t.id))
+            name = '{0} track {1}'.format(self.path, t.id)
+            label, decode = 'FLAC', flac.track_decoder(t.config, name)
+            fields = swr.audio_format(flac.FlacFile.from_bytes(t.config, name).bits_per_sample, swr.FLAC)
         else:
             label, decode = 'ALAC', alac.track_decoder(t.config)
-        return track_audio(self.path, t.id, label, lambda: self.frames(t), decode)
+            fields = swr.audio_format(alac.bit_depth(t.config), swr.ALAC)
+        return track_audio(self.path, t.id, label, lambda: self.frames(t), decode, **fields)
 
     def prefetch(self, payload_ids=(), time_ids=()):
         """Nothing to read ahead: the audio is read by WavStream, and there is no script or timestamp to read."""

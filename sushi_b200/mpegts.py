@@ -232,7 +232,10 @@ class TransportStream(object):
 
     def select_audio(self, track=None):
         s = self.select('audio', track)
-        return Audio(DECODED[audio_codec(s)][0], s.id, self.path, decode=lambda device: self._decode(device, s))
+        label = DECODED[audio_codec(s)][0]
+        # BD-LPCM's bit depth is in its PES headers, read on the GPU; TrueHD decodes to S32
+        return Audio(label, s.id, self.path, decode=lambda device: self._decode(device, s),
+                     fmt='S32' if label == 'TrueHD' else None)
 
     def _decode(self, device, s):
         """The BD-LPCM or TrueHD stream `s`, demuxed and decoded on the GPU (sb_ts_*).  The file is read in chunks of

@@ -63,7 +63,7 @@ class TrueHDFile(object):
 
     def select_audio(self, track=None):
         # one block holding every access unit; a negative file offset makes messages name each unit's own offset
-        return Audio('TrueHD', path=self.path, decode=lambda device: decode(
+        return Audio('TrueHD', path=self.path, fmt='S32', decode=lambda device: decode(
             device, self.data, np.zeros(1, np.int64), np.full(1, -1, np.int64)))
 
 

@@ -15,7 +15,7 @@ import zlib
 
 import numpy as np
 
-from . import _native, wavpack
+from . import _native, swr, wavpack
 from .common import Audio, SushiError
 from .flac import id3v2_size
 
@@ -123,7 +123,7 @@ class TTAFile(object):
         self.where = starts
 
     def select_audio(self, track=None):
-        return Audio('TTA', path=self.path, decode=self._decode)
+        return Audio('TTA', path=self.path, decode=self._decode, **swr.audio_format(self.bits, swr.TTA))
 
     def _decode(self, device):
         # the file's bytes as read, up to the end of the audio: frames at their file offsets, no copy

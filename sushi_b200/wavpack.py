@@ -15,7 +15,7 @@ import struct
 
 import numpy as np
 
-from . import _native
+from . import _native, swr
 from .common import Audio, SushiError
 
 WV_EXTENSIONS = ('.wv',)
@@ -232,7 +232,8 @@ class WavPackFile(object):
 
     def select_audio(self, track=None):
         return Audio('WavPack', path=self.path,
-                     decode=lambda device: decode(device, self.data, self.table, self.stream))
+                     decode=lambda device: decode(device, self.data, self.table, self.stream),
+                     **swr.audio_format(self.stream.bits_per_sample, swr.PLAIN))
 
 
 def decode(device, data, table, stream):

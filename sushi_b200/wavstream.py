@@ -21,7 +21,7 @@ import weakref
 
 import numpy as np
 
-from . import _native
+from . import _native, swr
 from ._nvtx import nvtx_range
 from .common import SushiError, clip, py2_round
 from .inputs import open_input, FlacFile, is_flac   # noqa: F401  (the FLAC reader stays importable from here)
@@ -96,13 +96,16 @@ class StreamGeometry(object):
 class WavStream(StreamGeometry):
     READ_CHUNK_SIZE = 1  # seconds per resample chunk (wav.py:105)
 
-    def __init__(self, path, sample_rate=12000, sample_type='uint8', device=None, loader='gpu', track=None):
+    def __init__(self, path, sample_rate=12000, sample_type='uint8', device=None, loader='gpu', track=None,
+                 ffmpeg_audio=False):
         """loader='gpu' (default): decode / resample / pad / normalise on the GPU (sb_load_pcm +
         sb_normalise); loader='host' runs the NumPy mirror of the same arithmetic and uploads the
         result (kept as the cross-check; both give bit-identical .data).  `path` is a file of any format in
         inputs.FORMATS, or an opened MatroskaFile, Mp4File or TransportStream (left open; a MatroskaFile's frames then
         come from one walk shared with the script and timecodes).  A container loads its audio stream `track` (a stream
-        id; None: the only audio track, else the default one, as the reference selects)."""
+        id; None: the only audio track, else the default one, as the reference selects).  ffmpeg_audio=True loads an
+        input that is not a RIFF WAV file as the mono `sample_rate` WAV the reference's ffmpeg call writes for it
+        (sushi_b200/swr.py); a WAV file loads as it always does."""
         if sample_type not in _DTYPES:
             raise SushiError('Unknown sample type of WAV stream, must be uint8 or float32')
         self._handle = None
@@ -110,7 +113,9 @@ class WavStream(StreamGeometry):
         reader, name = open_input(path)
         try:
             audio = reader.select_audio(track)
-            if audio.label is None:
+            if ffmpeg_audio and name != 'WAV':
+                self._load_ffmpeg(audio, sample_rate, sample_type, device, loader)
+            elif audio.label is None:
                 self._load_pcm(audio.pcm, sample_rate, sample_type, device, loader)
             else:
                 # compressed inputs are decoded on the GPU only
@@ -143,6 +148,21 @@ class WavStream(StreamGeometry):
             self._load_decoded(h, sample_rate, sample_type, device)
         else:
             self._load_gpu(data, frames, channels, width, rate, sample_rate, sample_type, device)
+
+    def _load_ffmpeg(self, audio, sample_rate, sample_type, device, loader):
+        """ffmpeg_audio=True: the reader's audio decoded (or container PCM uploaded) to an sb_pcm, converted by
+        sb_pcm_swr to the ffmpeg command line's mono `sample_rate` samples and loaded as their WAV loads."""
+        swr.check(audio)
+        if loader != 'gpu':
+            raise SushiError("{0}: --ffmpeg-audio needs loader='gpu'".format(audio.path))
+        if audio.label is None:
+            data, frames, channels, width, rate, big = audio.pcm()
+            buf = np.frombuffer(data, dtype=np.uint8)
+            h = _native.decode(device, 'sb_pcm_from_be' if big else 'sb_pcm_from_le',
+                               buf.ctypes.data_as(ctypes.c_void_p), frames, channels, width, rate)
+        else:
+            h = audio.decode(device)
+        self._load_decoded(swr.convert(device, h, audio, sample_rate), sample_rate, sample_type, device)
 
     def _load_decoded(self, h, sample_rate, sample_type, device, check=None):
         """_load_gpu_with on a decoder's sb_pcm handle `h` (sb_pcm_load), which it destroys; check(frames) may refuse
