@@ -65,17 +65,8 @@ extern "C" int sb_pcm_swr(const sb_pcm* in, uint64_t layout, int out_rate, sb_pc
     if (!sbswr::make_plan(layout, in->channels, in->rate, out_rate, in->frames, &p, msg, sizeof msg))
         SB_FAIL(SB_EINVAL, "%s: %s", who, msg);
     int tile = 256, width = 0;
-    if (p.resample) {
-        for (; tile >= 32; tile /= 2) {                      // the widest window any tile of `tile` outputs stages
-            const int64_t span = ((int64_t)(tile - 1) * p.rs.dst_incr / p.rs.src_incr) / p.rs.phase_count + 2;
-            if ((span + p.rs.filter_alloc) * (int64_t)sizeof(float) <= kSmemBytes) {
-                width = (int)(span + p.rs.filter_alloc);
-                break;
-            }
-        }
-        if (!width)
-            SB_FAIL(SB_EINVAL, "%s: sample rates %d -> %d need too wide a filter window", who, in->rate, out_rate);
-    }
+    if (p.resample && !sbswr::tile_shape(p.rs, kSmemBytes, &tile, &width))
+        SB_FAIL(SB_EINVAL, "%s: sample rates %d -> %d need too wide a filter window", who, in->rate, out_rate);
     int16_t* d_out = nullptr;
     float* d_bank = nullptr;
     SB_TRY(pool_alloc((void**)&d_out, sizeof(int16_t) * (size_t)p.out_frames + 16));

@@ -395,4 +395,23 @@ inline bool make_plan(uint64_t layout, int channels, int in_rate, int out_rate, 
     return true;
 }
 
+// The resample kernel's launch shape: the widest tile of 256, 128, 64 or 32 outputs whose input window fits in
+// max_bytes of shared memory, and that window's width in floats.  A tile of `tile` outputs starting at any t0 reads
+// samples s(t0) .. s(t0 + tile - 1) + filter_alloc - 1.  With X = (tile - 1) * dst_incr / src_incr (integer division)
+// the phase index p * phase_count + r (r < phase_count) of t0 advances by at most X + 1 over the tile, so
+// s(t0 + tile - 1) - s(t0) <= (r + X + 1) / phase_count <= X / phase_count + 1 = span - 1: the window has one float to
+// spare.  Returns false when even 32 outputs need a wider window (no rate pair make_resampler accepts does:
+// tests/test_swr_cases.py sweeps them).
+inline bool tile_shape(const Resampler& r, int max_bytes, int* tile, int* width) {
+    for (int t = 256; t >= 32; t /= 2) {
+        const int64_t span = ((int64_t)(t - 1) * r.dst_incr / r.src_incr) / r.phase_count + 2;
+        if ((span + r.filter_alloc) * (int64_t)sizeof(float) <= max_bytes) {
+            *tile = t;
+            *width = (int)(span + r.filter_alloc);
+            return true;
+        }
+    }
+    return false;
+}
+
 }  // namespace sbswr

@@ -4,7 +4,8 @@ ctypes on the libraries oracle/ref_flac.py loads.
 `demux(path)` gives the stream list (media type, codec name, default disposition), the chapters (start in seconds,
 from each chapter's own time base) and every packet (stream, bytes, file position).  `decode(path, sid, channels)`
 decodes one stream's packets, skipping a packet the decoder refuses as the ffmpeg command line does, and asserts
-the sample format it reads.  Struct offsets, as in tests/ref_mkv.py (libavformat / libavcodec 62):
+the sample format it reads; `decode_s16(path, sid)` also reads the decoder's channel layout and rate, for the
+--ffmpeg-audio oracle.  Struct offsets, as in tests/ref_mkv.py (libavformat / libavcodec 62):
     AVFormatContext.nb_streams +44, .streams +48, .nb_chapters +72, .chapters +80;
     AVStream.index +8, .codecpar +16, .disposition +64;  AVCodecParameters.codec_type +0, .codec_id +4;
     AVPacket.data +24, .size +32, .stream_index +36, .pos +72;  AVChapter.time_base +8, .start +16;
@@ -15,6 +16,7 @@ import ctypes
 import numpy as np
 
 from oracle import ref_flac
+from tests import ref_swr
 
 AVMEDIA_TYPES = {0: 'video', 1: 'audio', 2: 'data', 3: 'subtitles', 4: 'attachment'}
 AV_DISPOSITION_DEFAULT = 1
@@ -88,9 +90,26 @@ def demux(path, packets=True):
         fmt.avformat_close_input(ctypes.byref(ctx))
 
 
-def decode(path, sid, channels):
-    """-> (samples (n, channels) int64 as FFmpeg returns them, sample format, packets refused)."""
+def decoder_layout(dec):
+    """(channel mask, channel count) of an opened decoder context's `ch_layout` option.  A layout FFmpeg leaves
+    unspecified is the default layout of its channel count, as the ffmpeg command line assumes."""
+    _, _, util = ref_flac.libs()
+    util.av_opt_get_chlayout.argtypes = [ctypes.c_void_p, ctypes.c_char_p, ctypes.c_int,
+                                         ctypes.POINTER(ref_swr.ChLayout)]
+    util.av_channel_layout_default.argtypes = [ctypes.POINTER(ref_swr.ChLayout), ctypes.c_int]
+    layout = ref_swr.ChLayout()
+    assert util.av_opt_get_chlayout(dec, b'ch_layout', 0, ctypes.byref(layout)) >= 0
+    if layout.order != ref_swr.AV_CHANNEL_ORDER_NATIVE:
+        n = layout.nb_channels
+        layout = ref_swr.ChLayout()
+        util.av_channel_layout_default(ctypes.byref(layout), n)
+    return layout.mask, layout.nb_channels
+
+
+def _decode(path, sid, channels):
+    """-> (samples, sample format, packets refused, channel mask, sample rate); channels None: the decoder's"""
     fmt, codec, util = ref_flac.libs()
+    util.av_opt_get_int.argtypes = [ctypes.c_void_p, ctypes.c_char_p, ctypes.c_int, ctypes.POINTER(ctypes.c_int64)]
     ctx = _open(path)
     dec = pkt = frame = ctypes.c_void_p()
     chunks, sfmt, refused = [], None, 0
@@ -102,6 +121,8 @@ def decode(path, sid, channels):
         dec = ctypes.c_void_p(codec.avcodec_alloc_context3(c))
         assert codec.avcodec_parameters_to_context(dec, par) >= 0
         assert codec.avcodec_open2(dec, c, None) >= 0
+        if channels is None:
+            channels = decoder_layout(dec)[1]
         pkt = ctypes.c_void_p(codec.av_packet_alloc())
         frame = ctypes.c_void_p(util.av_frame_alloc())
 
@@ -129,6 +150,9 @@ def decode(path, sid, channels):
             codec.av_packet_unref(pkt)
         codec.avcodec_send_packet(dec, None)
         drain()
+        mask = decoder_layout(dec)[0]
+        rate = ctypes.c_int64()
+        assert util.av_opt_get_int(dec, b'ar', 0, ctypes.byref(rate)) >= 0
     finally:
         if frame:
             util.av_frame_free(ctypes.byref(frame))
@@ -138,7 +162,21 @@ def decode(path, sid, channels):
             codec.avcodec_free_context(ctypes.byref(dec))
         fmt.avformat_close_input(ctypes.byref(ctx))
     out = np.concatenate(chunks) if chunks else np.zeros((0, channels), np.int64)
-    return out, sfmt, refused
+    return out, sfmt, refused, mask, rate.value
+
+
+def decode(path, sid, channels):
+    """-> (samples (n, channels) int64 as FFmpeg returns them, sample format, packets refused)."""
+    return _decode(path, sid, channels)[:3]
+
+
+def decode_s16(path, sid):
+    """What the ffmpeg command line hands libswresample for stream `sid` of a source FFmpeg decodes to 16 bits:
+    (samples (n, channels) int16, the decoder's channel mask, its sample rate)."""
+    out, sfmt, _, mask, rate = _decode(path, sid, None)
+    assert sfmt in (1, 6), 'stream %d decodes to sample format %s, not S16' % (sid, sfmt)
+    assert bin(mask).count('1') == out.shape[1], (hex(mask), out.shape)
+    return out.astype(np.int16), mask, rate
 
 
 def decode_pcm(path, sid, channels, bits):

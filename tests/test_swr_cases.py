@@ -1,9 +1,11 @@
 """The --ffmpeg-audio conversion (sushi_b200/csrc/sb_swr.cuh) on the CPU, through tests/emu/emu_swr_driver.cpp compiled
 with g++, against libswresample itself (tests/ref_swr.py, its FMA3 path): the mono S16 output, its length included, bit
 for bit over input and output rates, layouts, lengths and values; the mono matrix row against swr_build_matrix2; the
-Kaiser window's Bessel function against av_bessel_i0; the float banks against their impulse read-outs.  Also pinned
-here: libswresample's output does not depend on how the input is chunked, remixing before resampling would give other
-samples, and its C, SSE and AVX paths stay within 1 LSB of the FMA3 path."""
+Kaiser window's Bessel function against av_bessel_i0; the float banks against their impulse read-outs.  The resample
+kernel's tiling on the CPU: sbswr::tile_shape's window against the one every output uses over about 440 rate pairs, and
+k_swr_resample's tiles and staged windows (emu_swr_convert_tiled) against the untiled loop at a pair of each tile
+size.  Also pinned here: libswresample's output does not depend on how the input is chunked, remixing before
+resampling would give other samples, and its C, SSE and AVX paths stay within 1 LSB of the FMA3 path."""
 import ctypes
 import os
 import subprocess
@@ -24,6 +26,15 @@ IN_RATES = [8000, 11025, 16000, 22050, 32000, 44100, 48000, 88200, 96000, 192000
 OUT_RATES = [12000, 8000, 24000, 44100, None]          # None: the input rate
 LAYOUTS = sorted(set(swr.DEFAULT.values()) | set(swr.FLAC.values()) | set(swr.ALAC.values()) | set(swr.TTA.values())
                  | {0x7, 0x33, 0x103, 0x603, 0x637, 0x60f, 0x3f, 0x63f})
+LENGTHS = [1, 2, 33, 65, 66, 67, 131, 132, 133, 200, 47999, 48000, 48001]
+SMEM_BYTES = 48 * 1024                                  # the shared memory sb_pcm_swr gives k_swr_resample's window
+# the sweep's grid beyond IN_RATES x OUT_RATES: exact and inexact (prime, off-by-one) rates
+GRID_IN = [1000, 2000, 4000, 7919, 8000, 11025, 12001, 16000, 22050, 24000, 32000, 44100, 44101, 48000, 64000, 88200,
+           96000, 96001, 128000, 176400, 192000, 192001, 256000, 352800, 384000, 384001, 512000, 705600, 767999, 768000]
+GRID_OUT = [1000, 2000, 4000, 4001, 6000, 8000, 11025, 12000, 12001, 16000, 22050, 24000, 32000, 44100, 48000]
+# a pair at each tile size k_swr_resample takes, and an inexact one at each narrow tile
+TILED = {(48000, 12000): 256, (44100, 12000): 256, (7919, 12000): 256, (192000, 4000): 128, (192001, 4001): 128,
+         (384000, 4000): 64, (384001, 4001): 64}
 
 
 @pytest.fixture(scope='module')
@@ -36,6 +47,8 @@ def emu():
     vp, i64, u64, i32, cp = ctypes.c_void_p, ctypes.c_int64, ctypes.c_uint64, ctypes.c_int, ctypes.c_char_p
     lib.emu_swr_plan.argtypes = [u64, i32, i32, i32, i64, vp, cp, i32]
     lib.emu_swr_convert.argtypes = [vp, i64, i32, u64, i32, i32, i32, vp, cp, i32]
+    lib.emu_swr_tiles.argtypes = [i32, i32, i32, i64, vp, cp, i32]
+    lib.emu_swr_convert_tiled.argtypes = [vp, i64, i32, u64, i32, i32, i32, vp, cp, i32]
     lib.emu_swr_bank.argtypes = [i32, i32, vp, cp, i32]
     lib.emu_swr_row.argtypes = [u64, vp, cp, i32]
     lib.emu_swr_bessel.argtypes = [ctypes.c_double]
@@ -57,6 +70,24 @@ def convert(emu, pcm, mask, in_rate, out_rate, mix_first=False):
     msg = ctypes.create_string_buffer(256)
     assert emu.emu_swr_convert(pcm.ctypes.data, len(pcm), pcm.shape[1], mask, in_rate, out_rate, int(mix_first),
                                out.ctypes.data, msg, 256) == 0, msg.value
+    return out[:int(g[0])]
+
+
+def tiles(emu, in_rate, out_rate, cap=1 << 26):
+    """-> (return code, [tile, width, largest window used, outputs walked, period], message) of emu_swr_tiles"""
+    g = np.zeros(5, np.int64)
+    msg = ctypes.create_string_buffer(256)
+    rc = emu.emu_swr_tiles(in_rate, out_rate, SMEM_BYTES, cap, g.ctypes.data, msg, 256)
+    return rc, [int(v) for v in g], msg.value.decode()
+
+
+def convert_tiled(emu, pcm, mask, in_rate, out_rate):
+    pcm = np.ascontiguousarray(pcm, np.int16)
+    g = plan(emu, mask, pcm.shape[1], in_rate, out_rate, len(pcm))
+    out = np.zeros(int(g[0]) + 1, np.int16)
+    msg = ctypes.create_string_buffer(256)
+    assert emu.emu_swr_convert_tiled(pcm.ctypes.data, len(pcm), pcm.shape[1], mask, in_rate, out_rate, SMEM_BYTES,
+                                     out.ctypes.data, msg, 256) == 0, msg.value
     return out[:int(g[0])]
 
 
@@ -97,7 +128,7 @@ def test_layouts(emu, mask, rates):
     check(emu, signal('noise', rates[0] // 2 + 7, ch, rates[0], mask), mask, *rates)
 
 
-@pytest.mark.parametrize('frames', [1, 2, 33, 65, 66, 67, 131, 132, 133, 200, 47999, 48000, 48001])
+@pytest.mark.parametrize('frames', LENGTHS)
 @pytest.mark.parametrize('rates', [(48000, 12000), (8000, 12000), (7919, 12000), (44100, 44100)], ids=str)
 def test_lengths(emu, frames, rates):
     check(emu, signal('noise', frames, 2, rates[0], frames), 0x3, *rates)
@@ -114,6 +145,48 @@ def test_values(emu, kind, mask, rates):
 def test_tens_of_seconds(emu):
     check(emu, signal('noise', 44100 * 20 + 3, 2, 44100, 7), 0x3, 44100, 12000)
     check(emu, signal('tone', 48000 * 12, 6, 48000, 8), 0x3f, 48000, 12000)
+
+
+def test_tile_windows_cover_every_output(emu):
+    """sbswr::tile_shape's window against the window every output of every tile uses, for every resampling pair of
+    IN_RATES x OUT_RATES and of a grid from 1 kHz to 768 kHz in and 1 kHz to 48 kHz out.  sbswr::position is walked
+    over lcm(period, tile) outputs, after which both the position pattern and the tile starts repeat, so every tile
+    start is seen against every phase of the pattern.  The window fits in shared memory and covers each output's taps
+    with the one float to spare the header derives; tiles of 256, 128 and 64 outputs all occur, and no pair
+    make_resampler accepts reaches the "too wide a filter window" refusal (the guard stays in the library)."""
+    pairs = {(a, b or a) for a in IN_RATES for b in OUT_RATES} | {(a, b) for a in GRID_IN for b in GRID_OUT}
+    counts, slack, refused, outputs = {}, [], 0, 0
+    for a, b in sorted(p for p in pairs if p[0] != p[1]):
+        rc, (tile, width, need, walked, period), msg = tiles(emu, a, b)
+        if rc == -1:
+            assert 'are not supported' in msg, msg
+            refused += 1
+            continue
+        assert rc == 0, (a, b, msg)
+        assert walked % period == 0 and walked % tile == 0, (a, b, walked, period, tile)
+        assert need <= width and width * 4 <= SMEM_BYTES, (a, b, tile, width, need)
+        counts[tile] = counts.get(tile, 0) + 1
+        slack.append(width - need)
+        outputs += walked
+    print('pairs by tile:', counts, '; refused by make_resampler:', refused, '; outputs walked:', outputs)
+    assert counts.get(256) and counts.get(128) and counts.get(64), counts
+    assert min(slack) == 1, min(slack)
+
+
+def test_a_refused_pair_has_no_tile(emu):
+    rc, _, msg = tiles(emu, 768000, 2000)
+    assert rc == -1 and 'sample rates 768000 -> 2000 are not supported' in msg
+
+
+@pytest.mark.parametrize('frames', LENGTHS)
+@pytest.mark.parametrize('rates', sorted(TILED), ids=str)
+def test_tiled_is_untiled(emu, rates, frames):
+    """emu_swr_convert_tiled (k_swr_resample's tiles, staged windows and channel order, every window read checked)
+    equals emu_swr_convert bit for bit, at a pair of each tile size"""
+    assert tiles(emu, *rates)[1][0] == TILED[rates]
+    pcm = signal('noise', frames, 3, rates[0], frames)
+    want = convert(emu, pcm, 0x7, *rates)
+    assert np.array_equal(convert_tiled(emu, pcm, 0x7, *rates), want)
 
 
 def test_full_scale_reaches_the_clip(emu):

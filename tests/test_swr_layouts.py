@@ -11,7 +11,7 @@ import pytest
 from oracle import ref_flac
 from sushi_b200 import SushiError, inputs
 from tests import flac_cases, mkv_alac_cases, mkv_cases, mkv_tta_cases, mkv_wavpack_cases, mp4_cases
-from tests import ref_mp4, ref_swr, ts_cases, tta_cases, wavpack_cases
+from tests import ref_mp4, ts_cases, tta_cases, wavpack_cases
 
 S16, S16P, S32, S32P = 1, 6, 2, 7
 FMT = {S16: 'S16', S16P: 'S16', S32: 'S32', S32P: 'S32'}
@@ -21,10 +21,6 @@ COMPARED = set()
 def ffmpeg_audio(path):
     """{stream id: (sample format, channel mask)} of each audio stream FFmpeg decodes a frame of"""
     fmt, codec, util = ref_flac.libs()
-    ref_swr.lib()
-    util.av_opt_get_chlayout.argtypes = [ctypes.c_void_p, ctypes.c_char_p, ctypes.c_int,
-                                         ctypes.POINTER(ref_swr.ChLayout)]
-    util.av_channel_layout_default.argtypes = [ctypes.POINTER(ref_swr.ChLayout), ctypes.c_int]
     streams = ref_mp4.demux(path, packets=False).streams
     out = {}
     for sid, (kind, _, _) in enumerate(streams):
@@ -51,13 +47,7 @@ def ffmpeg_audio(path):
                 codec.av_packet_unref(pkt)
             if not got:
                 continue
-            sfmt, layout = ref_mp4._i32(frame.value + 116), ref_swr.ChLayout()      # AVFrame.format
-            assert util.av_opt_get_chlayout(dec, b'ch_layout', 0, ctypes.byref(layout)) >= 0
-            if layout.order != ref_swr.AV_CHANNEL_ORDER_NATIVE:
-                n = layout.nb_channels
-                layout = ref_swr.ChLayout()
-                util.av_channel_layout_default(ctypes.byref(layout), n)
-            out[sid] = (FMT.get(sfmt), layout.mask, layout.nb_channels)
+            out[sid] = (FMT.get(ref_mp4._i32(frame.value + 116)),) + ref_mp4.decoder_layout(dec)   # AVFrame.format
         finally:
             if frame:
                 util.av_frame_free(ctypes.byref(frame))
