@@ -39,7 +39,7 @@
 extern "C" {
 #endif
 
-#define SB_ABI_VERSION 12
+#define SB_ABI_VERSION 13
 
 /* status codes */
 #define SB_OK            0
@@ -323,6 +323,16 @@ int sb_wavpack_decode_blocks(const void* buf, int64_t nbytes, const int64_t* tab
 int sb_tta_decode_frames(const void* buf, int64_t nbytes, const int64_t* offsets, const int64_t* file_offsets, int64_t n,
                          const int32_t* config, sb_pcm** out);
 
+/* MPEG-1/2 audio layer II, MP2 (ABI version 13): FFmpeg's fixed-point `mp2` decoder output, bit for bit, 1 or 2
+ * channels at 16 to 48 kHz.  `buf` holds a Matroska track's block payloads back to back (block k at offsets[k], at
+ * file offset file_offsets[k]).  FFmpeg decodes each block as a packet, so every block must start with a frame header
+ * and hold whole frames; a last frame cut short is decoded with zeros for its missing bits, as FFmpeg decodes it.
+ * Refused with SB_EINVAL, naming the frame and the file offset of its block: layer I or III, MPEG-2.5, free format, a
+ * reserved bitrate, rate or emphasis, a broken sync, a change of layer, rate or channel count (bitrates may change), a
+ * CRC-16 that disagrees, a frame whose samples run past its end, a frame that straddles blocks. */
+int sb_mp2_decode_frames(const void* buf, int64_t nbytes, const int64_t* offsets, const int64_t* file_offsets,
+                         int64_t n, sb_pcm** out);
+
 /* ---- MPEG transport streams (ABI version 7) ----------------------------------
  *
  * One audio PID of a BDAV (192-byte packets: a 4-byte arrival time stamp, then the 188-byte packet) or plain
@@ -339,7 +349,11 @@ int sb_tta_decode_frames(const void* buf, int64_t nbytes, const int64_t* offsets
  *                     refused, as FFmpeg's decoder refuses them;
  *   SB_TS_TRUEHD      the payloads of the PES packets FFmpeg routes to the TrueHD stream (every stream_id_extension
  *                     but 0x76, the AC-3 sub-stream) are one raw TrueHD stream, decoded as sb_truehd_decode decodes a
- *                     .thd file; AUs may straddle PES and TS packets.
+ *                     .thd file; AUs may straddle PES and TS packets;
+ *   SB_TS_MP2         (ABI version 13) the PES payloads are one MPEG audio stream, decoded as sb_mp2_decode_frames
+ *                     decodes a track's blocks, but as one stream split at its headers, as FFmpeg's parser splits it:
+ *                     bytes before the first header take the first whole frame with them (FFmpeg's decoder refuses
+ *                     that packet), and a last frame cut short is decoded with zeros and sets *cut.
  * Damage fails with SB_EINVAL, sb_last_error() naming the byte offset of the packet (TS damage), of the PES's first
  * packet (PES damage) or of the packet holding an AU's first byte (TrueHD damage).  A last PES shorter than its
  * PES_packet_length (a cut file) keeps its whole sample frames and sets *cut; one cut inside its header is dropped.
@@ -347,6 +361,7 @@ int sb_tta_decode_frames(const void* buf, int64_t nbytes, const int64_t* offsets
  * outlives the sb_ts. */
 #define SB_TS_PCM_BLURAY 0
 #define SB_TS_TRUEHD 1
+#define SB_TS_MP2 2
 int sb_ts_open(int packet_size, int32_t pid, int32_t codec, sb_ts** out);
 int sb_ts_feed(sb_ts* ts, const void* host_chunk, int64_t nbytes, int64_t file_offset);
 int sb_ts_finish(sb_ts* ts, int32_t* cut, sb_pcm** out);

@@ -145,6 +145,10 @@ int pcm_handle(int16_t* d_pcm, int64_t frames, int channels, int rate, sb_pcm** 
 
 // sb_truehd.cu: sb_truehd_decode on a stream already on the device (sb_ts.cu feeds it a transport stream's TrueHD
 // payload); where(off) names the file offset of stream byte `off` in messages
+// MP2 (sb_mp2.cu): the stream in `host` and on the device at d_buf (zero tail of sb_decode.h); where(b) the file
+// offset of stream byte b; *cut 1 when a cut last frame was dropped
+int mp2_decode(const uint8_t* host, const uint8_t* d_buf, int64_t nbytes, const std::function<int64_t(int64_t)>& where,
+               int32_t* cut, sb_pcm** out);
 int truehd_index_device(const uint8_t* host, const uint8_t* d_buf, int64_t nbytes, const int64_t* offsets,
                         const int64_t* d_blocks, int64_t n, const std::function<int64_t(int64_t)>& where, sb_pcm** out);
 

@@ -171,6 +171,10 @@ k_pes_index(const uint8_t* __restrict__ es, int64_t es_total, const PesStart* __
     if (p.code) { fail_at(err, where, p.code); return; }
     if (p.cut) atomicOr(&misc[1], 1u);
     if (p.cut == 2) return;                            // cut inside its header: dropped
+    if (codec == SB_TS_MP2) {
+        count[s] = p.payload_len;
+        return;
+    }
     if (codec == SB_TS_TRUEHD) {
         count[s] = p.ext_id == 0x76 ? 0 : p.payload_len;
         return;
@@ -294,7 +298,7 @@ int sb_ts_open(int packet_size, int32_t pid, int32_t codec, sb_ts** out) {
     if (!out) SB_FAIL(SB_EINVAL, "sb_ts_open: NULL argument");
     if (packet_size != 188 && packet_size != 192) SB_FAIL(SB_EINVAL, "sb_ts_open: packet size %d (188 or 192)", packet_size);
     if (pid < 0 || pid > 0x1FFE) SB_FAIL(SB_EINVAL, "sb_ts_open: PID %d", pid);
-    if (codec != SB_TS_PCM_BLURAY && codec != SB_TS_TRUEHD) SB_FAIL(SB_EINVAL, "sb_ts_open: codec %d", codec);
+    if (codec != SB_TS_PCM_BLURAY && codec != SB_TS_TRUEHD && codec != SB_TS_MP2) SB_FAIL(SB_EINVAL, "sb_ts_open: codec %d", codec);
     sb_ts* t = new (std::nothrow) sb_ts();
     if (!t) SB_FAIL(SB_ENOMEM, "sb_ts_open: out of host memory");
     t->psize = packet_size; t->pid = pid; t->codec = codec;
@@ -460,8 +464,8 @@ int sb_ts_finish(sb_ts* t, int32_t* cut, sb_pcm** out) {
         SB_TRY(cuda_result(e, who));
         return pcm_handle(blocks.take(d_pcm), total, f.channels, f.rate, out);
     }
-    // TrueHD: the kept payloads back to back, then the .thd decoder on them as one block
-    if (total < 1) SB_FAIL(SB_EINVAL, "PID %d carries no TrueHD payload", t->pid);
+    // TrueHD and MP2: the kept payloads back to back, then the decoder on them as one stream
+    if (total < 1) SB_FAIL(SB_EINVAL, "PID %d carries no %s payload", t->pid, t->codec == SB_TS_MP2 ? "MP2" : "TrueHD");
     uint8_t* d_thd = nullptr;
     int64_t* d_len = nullptr;
     int64_t* d_block = nullptr;
@@ -502,6 +506,12 @@ int sb_ts_finish(sb_ts* t, int32_t* cut, sb_pcm** out) {
                           - tab.begin() - 1;
         return k >= 0 ? tab[(size_t)k].file_off : -1;
     };
+    if (t->codec == SB_TS_MP2) {
+        int32_t dropped = 0;
+        SB_TRY(mp2_decode(host.data(), d_thd, total, where, &dropped, out));
+        *cut = *cut || dropped;
+        return SB_OK;
+    }
     const int64_t zero = 0;
     return truehd_index_device(host.data(), d_thd, total, &zero, d_block, 1, where, out);
 }

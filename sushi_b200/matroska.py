@@ -707,6 +707,11 @@ class MatroskaFile(object):
         elif kind == 'tta':
             label, decode = 'TTA', tta.track_decoder(t, self.timestamp_scale, self.duration)
             fields = swr.audio_format(t.bit_depth, swr.TTA)
+        elif kind == 'mp2':
+            # every block must hold whole frames: FFmpeg decodes each block as a packet
+            label, fields = 'MP2', swr.audio_format(16, swr.PLAIN)
+            decode = lambda device, table: _native.decode_frames(device, 'sb_mp2_decode_frames', table.data,
+                                                                 table.offset, table.block)
         else:
             label, decode, fields = 'TrueHD', decode_truehd, {'fmt': 'S32'}
         return track_audio(self.path, t.id, label, read_frames, decode, **fields)
@@ -751,9 +756,9 @@ class MatroskaFile(object):
 
 
 def audio_codec(track):
-    """'flac', 'truehd', 'alac', 'wavpack', 'tta' or 'pcm' for an audio track the GPU loader decodes (FLAC, Dolby
+    """'flac', 'truehd', 'alac', 'wavpack', 'tta', 'mp2' or 'pcm' for an audio track the GPU loader decodes (FLAC, Dolby
     TrueHD, ALAC, whose CodecPrivate is the ALACSpecificConfig, WavPack stream versions 0x402-0x410, TTA of 16 or 24
-    bits and 1 to 8 channels, little-endian integer PCM of 16 or 24 bits);
+    bits and 1 to 8 channels, MPEG audio layer II, little-endian integer PCM of 16 or 24 bits);
     SushiError naming the track and its codec for anything else."""
     if track.refusal:
         raise SushiError(track.refusal)
@@ -771,9 +776,11 @@ def audio_codec(track):
     if track.codec_id == 'A_TTA1':
         tta.check_track(track)
         return 'tta'
+    if track.codec_id == 'A_MPEG/L2':
+        return 'mp2'
     what = track.codec_id + (' at {0} bits'.format(track.bit_depth) if track.codec_id.startswith('A_PCM') else '')
     raise SushiError('Audio track {0} is {1}, which cannot be decoded here (FLAC, TrueHD, ALAC, WavPack, TTA and 16- or '
-                     '24-bit little-endian PCM can): convert it to FLAC or WAV first'.format(track.id, what))
+                     '24-bit little-endian PCM can, and MPEG audio layer II): convert it to FLAC or WAV first'.format(track.id, what))
 
 
 def _ass_time(ns):

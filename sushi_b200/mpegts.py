@@ -23,7 +23,7 @@ import os
 
 import numpy as np
 
-from . import _native
+from . import _native, swr
 from ._nvtx import nvtx_range
 from .common import Audio, SushiError, select_stream
 
@@ -43,7 +43,10 @@ HDMV_TYPES = {0x80: ('audio', 'pcm_bluray'), 0x81: ('audio', 'ac3'), 0x82: ('aud
               0xA2: ('audio', 'dts'), 0x90: ('subtitles', 'hdmv_pgs_subtitle'),
               0x92: ('subtitles', 'hdmv_text_subtitle')}
 MISC_TYPES = {0x81: ('audio', 'ac3'), 0x8A: ('audio', 'dts')}
-DECODED = {'pcm_bluray': ('BD-LPCM', _native.SB_TS_PCM_BLURAY), 'truehd': ('TrueHD', _native.SB_TS_TRUEHD)}
+# stream types 0x03 and 0x04 are listed as `mp3` until FFmpeg's parser reads a frame header; the GPU decodes layer II
+# and refuses layer I and III by name
+DECODED = {'pcm_bluray': ('BD-LPCM', _native.SB_TS_PCM_BLURAY), 'truehd': ('TrueHD', _native.SB_TS_TRUEHD),
+           'mp3': ('MP2', _native.SB_TS_MP2)}
 
 
 def is_transport_stream(path):
@@ -233,12 +236,12 @@ class TransportStream(object):
     def select_audio(self, track=None):
         s = self.select('audio', track)
         label = DECODED[audio_codec(s)][0]
-        # BD-LPCM's bit depth is in its PES headers, read on the GPU; TrueHD decodes to S32
-        return Audio(label, s.id, self.path, decode=lambda device: self._decode(device, s),
-                     fmt='S32' if label == 'TrueHD' else None)
+        # BD-LPCM's bit depth is in its PES headers, read on the GPU; TrueHD decodes to S32, MP2 to S16
+        fields = swr.audio_format(16, swr.PLAIN) if label == 'MP2' else {'fmt': 'S32' if label == 'TrueHD' else None}
+        return Audio(label, s.id, self.path, decode=lambda device: self._decode(device, s), **fields)
 
     def _decode(self, device, s):
-        """The BD-LPCM or TrueHD stream `s`, demuxed and decoded on the GPU (sb_ts_*).  The file is read in chunks of
+        """The BD-LPCM, TrueHD or MP2 stream `s`, demuxed and decoded on the GPU (sb_ts_*).  The file is read in chunks of
         CHUNK_BYTES into two page-locked buffers, one after the other, so that the GPU scans one chunk while the next
         is read."""
         lib = _native.lib(device)
@@ -263,9 +266,9 @@ class TransportStream(object):
 
 
 def audio_codec(stream):
-    """'pcm_bluray' or 'truehd' for a stream the GPU decodes; SushiError naming the stream and FFmpeg's codec name
+    """'pcm_bluray', 'truehd' or 'mp3' (MPEG audio: layer II is decoded) for a stream the GPU decodes; SushiError naming the stream and FFmpeg's codec name
     for anything else."""
     if stream.codec in DECODED:
         return stream.codec
-    raise SushiError('Audio track {0} is {1}, which cannot be decoded here (BD-LPCM and TrueHD can): convert it to '
+    raise SushiError('Audio track {0} is {1}, which cannot be decoded here (BD-LPCM, TrueHD and MP2 can): convert it to '
                      'FLAC or WAV first'.format(stream.id, stream.codec))
