@@ -39,7 +39,7 @@
 extern "C" {
 #endif
 
-#define SB_ABI_VERSION 13
+#define SB_ABI_VERSION 14
 
 /* status codes */
 #define SB_OK            0
@@ -55,6 +55,7 @@ extern "C" {
 typedef struct sb_stream sb_stream;      /* opaque: one normalised stream in HBM */
 typedef struct sb_pcm sb_pcm;            /* opaque: decoded interleaved int16 PCM on the device */
 typedef struct sb_ts sb_ts;              /* opaque: one audio PID of an MPEG transport stream being demuxed */
+typedef struct sb_ps sb_ps;              /* opaque: one audio stream of an MPEG program stream being demuxed */
 
 /* ---- life cycle ------------------------------------------------------- */
 
@@ -332,6 +333,12 @@ int sb_tta_decode_frames(const void* buf, int64_t nbytes, const int64_t* offsets
  * CRC-16 that disagrees, a frame whose samples run past its end, a frame that straddles blocks. */
 int sb_mp2_decode_frames(const void* buf, int64_t nbytes, const int64_t* offsets, const int64_t* file_offsets,
                          int64_t n, sb_pcm** out);
+/* One MPEG audio stream as a raw .mp2 file holds it (ABI version 14): `buf` the bytes between the file's tags, which
+ * start at file offset `file_offset`.  Split at its headers as FFmpeg's parser splits it, with SB_TS_MP2's rules: bytes
+ * before the first header take the first whole frame with them (FFmpeg's decoder refuses that packet), and a last frame
+ * cut short is decoded with zeros and sets *cut.  Refusals as sb_mp2_decode_frames's, naming the frame's own file
+ * offset. */
+int sb_mp2_decode_stream(const void* buf, int64_t nbytes, int64_t file_offset, int32_t* cut, sb_pcm** out);
 
 /* ---- MPEG transport streams (ABI version 7) ----------------------------------
  *
@@ -366,6 +373,25 @@ int sb_ts_open(int packet_size, int32_t pid, int32_t codec, sb_ts** out);
 int sb_ts_feed(sb_ts* ts, const void* host_chunk, int64_t nbytes, int64_t file_offset);
 int sb_ts_finish(sb_ts* ts, int32_t* cut, sb_pcm** out);
 int sb_ts_destroy(sb_ts* ts);
+
+/* ---- MPEG program streams (ABI version 14) ------------------------------------
+ *
+ * One MPEG audio stream (stream id 0xC0 to 0xDF; substream_id -1) of an MPEG-1 or MPEG-2 program stream (VCD and SVCD
+ * .mpg, DVD .vob, DVB recordings), demuxed on the GPU and decoded as SB_TS_MP2 decodes a PID.  The file is fed in
+ * chunks of any size, in order; the host does no per-packet work.  Packets (pack headers, system headers, PSM, padding,
+ * private streams, PES) have variable lengths and may straddle chunks: every start code of a chunk is found, each
+ * links to the one its packet's length reaches, and the chain from the position the previous chunk reached is found by
+ * pointer jumping over those links; start codes inside payloads lie off the chain.  The chosen stream's PES headers
+ * (MPEG-1: stuffing, STD buffer, PTS / DTS; MPEG-2: flags and header length) are parsed and their payloads appended
+ * to the elementary stream, which sb_ps_finish decodes; messages about a frame name the file offset of the PES holding
+ * its header.  Damage fails with SB_EINVAL naming the byte offset: a position the chain reaches that holds no start
+ * code (a broken start code, a wrong length, bytes between packets), an invalid pack header, an invalid PES header of
+ * the chosen stream.  A last PES cut by the file's end keeps its bytes and sets *cut; one cut inside its header is
+ * dropped.  sb_ps_feed returns once the chunk is copied and scanned for start codes.  The sb_pcm outlives the sb_ps. */
+int sb_ps_open(int32_t stream_id, int32_t substream_id, sb_ps** out);
+int sb_ps_feed(sb_ps* ps, const void* host_chunk, int64_t nbytes, int64_t file_offset);
+int sb_ps_finish(sb_ps* ps, int32_t* cut, sb_pcm** out);
+int sb_ps_destroy(sb_ps* ps);
 
 /* ---- multi-GPU: events shard across ranks (SURVEY.md 8e) ---------------- */
 

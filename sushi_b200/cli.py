@@ -1,7 +1,7 @@
 """The Sushi command line: `python -m sushi_b200 --src a.mkv --dst b.mkv -o out.ass`.
 
 Flags, defaults and checks are the reference's (sushi.py:528-843).  --src and --dst are files of the formats in
-inputs.FORMATS, taken by their extensions.  For a WAV file the reference starts no subprocess either; any other
+inputs.READERS, taken by their extensions.  For a WAV file the reference starts no subprocess either; any other
 format is decoded on the GPU, where the reference would have ffmpeg convert it to a WAV file (DESIGN.md section 2):
 no WAV file is ever written.  A Matroska input also gives, as the reference's ffmpeg and
 mkvextract calls do, the script, the chapters and the video timestamps (sushi_b200.matroska); those are written to
@@ -17,7 +17,7 @@ import time
 
 from . import __version__, swr
 from .common import SushiError
-from .inputs import FORMATS
+from .inputs import READERS
 from .pipeline import shift_script
 from .script import format_srt_time
 from .timing import get_ogm_start_times, get_xml_start_times, load_keyframe_times
@@ -122,17 +122,18 @@ def create_arg_parser():
 
 
 def _open_input(path):
-    """The opened reader of a container input (inputs.FORMATS: Matroska, MP4, transport stream), which also gives its
-    script, chapters and streams; None for a WAV, FLAC, raw TrueHD (.thd), raw WavPack (.wv) or raw TTA (.tta) input,
+    """The opened reader of a container input (inputs.READERS: Matroska, MP4, transport or program stream), which also
+    gives its script, chapters and streams; None for a WAV, FLAC, raw TrueHD (.thd), WavPack (.wv), TTA (.tta) or MPEG
+    audio (.mp2, .mpa, .m2a) input,
     which WavStream reads.  Any other extension, or a container's that does not open as one, is refused where the
     reference would have ffmpeg demux it."""
     ext = get_extension(path)
-    fmt = next((f for f in FORMATS if ext in f.extensions), None)
+    fmt = next((f for f in READERS if ext in f.extensions), None)
     refusal = '{0}: demuxing is not supported, convert the input to WAV or FLAC first'.format(path)
     if fmt is None:
         raise SushiError(refusal)
     if fmt.opens_as is None:
-        if fmt.name in ('WavPack', 'TTA'):
+        if fmt.name in ('WavPack', 'TTA', 'MPEG audio'):
             fmt.reader(path)                       # its refusals, before the GPU is touched
         return None
     try:

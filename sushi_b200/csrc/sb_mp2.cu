@@ -247,4 +247,15 @@ int sb_mp2_decode_frames(const void* buf, int64_t nbytes, const int64_t* offsets
     return mp2_decode(host, d_buf, nbytes, where, &cut, out);
 }
 
+int sb_mp2_decode_stream(const void* buf, int64_t nbytes, int64_t file_offset, int32_t* cut, sb_pcm** out) {
+    const char* who = "sb_mp2_decode_stream";
+    SB_TRY(entry_check(who, buf && cut && out));
+    if (nbytes < 1 || file_offset < 0) SB_FAIL(SB_EINVAL, "sb_mp2_decode_stream: bad stream parameters");
+    const uint8_t* host = static_cast<const uint8_t*>(buf);
+    Blocks blocks;
+    uint8_t* d_buf = nullptr;
+    SB_TRY(upload_padded(blocks, &d_buf, host, nbytes, who));
+    return mp2_decode(host, d_buf, nbytes, [&](int64_t b) { return file_offset + b; }, cut, out);
+}
+
 }  // extern "C"

@@ -3,12 +3,12 @@ them all) with one method, select_audio(track=None), which makes every refusal t
 common.Audio WavStream loads.  WavStream detects the format (open_input); the command line goes by file extension."""
 import collections
 
-from . import matroska, mp4, mpegts, truehd, tta, wavpack
+from . import matroska, mp4, mpa, mpegps, mpegts, truehd, tta, wavpack
 from .flac import FlacFile, is_flac
 from .wav import DownmixedWavFile
 
 # name: as the log names it; extensions: what the command line takes it by; sniff(path): whether a file is one (by its
-# content; a transport stream and a TrueHD stream by its name), asked in the table's order; reader: its class; opens_as:
+# content; a transport stream, a program stream, raw MPEG audio and a TrueHD stream by its name), asked in the table's order; reader: its class; opens_as:
 # for a container, whose script, chapters and streams the command line reads too, what its extensions must open as.
 Format = collections.namedtuple('Format', 'name extensions sniff reader opens_as')
 FORMATS = (
@@ -22,14 +22,22 @@ FORMATS = (
     Format('FLAC', ('.flac',), is_flac, FlacFile, None),
     Format('WAV', ('.wav',), lambda path: True, DownmixedWavFile, None),      # whatever is nothing else
 )
+# The MPEG systems whose audio is MP2: program streams and raw MPEG audio, both known by their names.  They are asked
+# before the table above; READERS is the whole table, in the order open_input asks.
+MPEG_FORMATS = (
+    Format('program stream', mpegps.PS_EXTENSIONS, mpegps.is_program_stream, mpegps.ProgramStream,
+           'a program stream'),
+    Format('MPEG audio', mpa.MPA_EXTENSIONS, mpa.is_mpeg_audio, mpa.MpegAudioFile, None),
+)
+READERS = MPEG_FORMATS + FORMATS
 
 
 def open_input(source):
     """(reader, format name) of `source`: a file name, whose format is detected by content, or an opened container
-    reader (MatroskaFile, Mp4File, TransportStream), which is returned as it is and never sniffed."""
-    for f in FORMATS:
+    reader (MatroskaFile, Mp4File, TransportStream, ProgramStream), which is returned as it is and never sniffed."""
+    for f in READERS:
         if f.opens_as and isinstance(source, f.reader):
             return source, f.name
-    for f in FORMATS:
+    for f in READERS:
         if f.sniff(source):
             return f.reader(source), f.name

@@ -95,7 +95,7 @@ def _resolve_links(events):
 
 def shift_script(src_audio, dst_audio, script_path, output_path, sample_rate=12000, sample_type='uint8',
                  chapter_times=(), src_track=None, dst_track=None, ffmpeg_audio=False, **options):
-    """src/dst audio (whatever WavStream takes: a file of a format in inputs.FORMATS, or an opened container reader) +
+    """src/dst audio (whatever WavStream takes: a file of a format in inputs.READERS, or an opened container reader) +
     ASS/SRT script in, shifted script out (the audio-in/script-out core of the CLI).
     src_track / dst_track are the audio stream ids of container inputs (None: the reference's default rule).
     ffmpeg_audio loads inputs other than WAV files as the reference's ffmpeg call writes them (WavStream).

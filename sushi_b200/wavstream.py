@@ -101,7 +101,7 @@ class WavStream(StreamGeometry):
         """loader='gpu' (default): decode / resample / pad / normalise on the GPU (sb_load_pcm +
         sb_normalise); loader='host' runs the NumPy mirror of the same arithmetic and uploads the
         result (kept as the cross-check; both give bit-identical .data).  `path` is a file of any format in
-        inputs.FORMATS, or an opened MatroskaFile, Mp4File or TransportStream (left open; a MatroskaFile's frames then
+        inputs.READERS, or an opened MatroskaFile, Mp4File or TransportStream (left open; a MatroskaFile's frames then
         come from one walk shared with the script and timecodes).  A container loads its audio stream `track` (a stream
         id; None: the only audio track, else the default one, as the reference selects).  ffmpeg_audio=True loads an
         input that is not a RIFF WAV file as the mono `sample_rate` WAV the reference's ffmpeg call writes for it
