@@ -182,6 +182,44 @@ def decode_frames(device, name, data, offsets, blocks, *args):
                   blocks.ctypes.data_as(c_i64p), len(offsets), *args)
 
 
+def demux_file(device, prefix, open_args, path, chunk_bytes, align=1):
+    """The file at `path` demuxed and decoded on the GPU by a chunked demultiplexer (`prefix` 'sb_ts' or 'sb_ps'):
+    <prefix>_open(*open_args), the file fed in chunks of chunk_bytes rounded down to whole `align`-byte packets,
+    <prefix>_finish, and <prefix>_destroy however that ends.  Returns (sb_pcm handle, the cut flag finish set, the bytes
+    of a partial last packet, which are not fed).  Every chunk goes through one page-locked buffer: a feed returns only
+    once its chunk has been copied to the device (include/sushi_b200.h), so the buffer can be refilled while the GPU
+    scans it."""
+    l = lib(device)
+    t = c_vp()
+    check(getattr(l, prefix + '_open')(*open_args, ctypes.byref(t)), prefix + '_open')
+    feed = getattr(l, prefix + '_feed')
+    cut = ctypes.c_int32()
+    try:
+        size = max(align, chunk_bytes // align * align)
+        buf = pinned_empty((size,), np.uint8)
+        view = memoryview(buf)
+        pos = 0
+        with nvtx_range('sushi_b200: ' + prefix + '_feed'), open(path, 'rb', buffering=0) as f:
+            while True:
+                got = 0
+                while got < size:
+                    r = f.readinto(view[got:])
+                    if not r:
+                        break
+                    got += r
+                whole = got - got % align
+                if whole:
+                    check(feed(t, buf.ctypes.data_as(c_vp), whole, pos), prefix + '_feed')
+                pos += whole
+                if got < size:
+                    break
+        del view, buf
+        h = decode(device, prefix + '_finish', t, ctypes.byref(cut))
+    finally:
+        getattr(l, prefix + '_destroy')(t)
+    return h, cut.value, got - whole
+
+
 def pinned_empty(shape, dtype):
     """numpy array over page-locked host memory (freed when the array is garbage collected)."""
     import weakref

@@ -43,6 +43,35 @@ def format_stream(t):
     return '{0}{1}: {2}'.format(t.id, ' (%s)' % t.title if t.title else '', t.info)
 
 
+class Container(object):
+    """What every container reader (Matroska, MP4, transport and program streams) offers over its stream list
+    `self.tracks` (objects with .id, .kind, .title, .info and .default) and the file name `self.path`."""
+
+    def close(self):
+        pass
+
+    def __enter__(self):
+        return self
+
+    def __exit__(self, *exc):
+        self.close()
+
+    def prefetch(self, payload_ids=(), time_ids=()):
+        """Nothing to read ahead: the audio is read by WavStream, and there is no script or timestamp to read."""
+
+    @property
+    def streams_all(self):
+        """Every stream of the file, in its order (the MPEG readers' name for `tracks`)."""
+        return self.tracks
+
+    def streams(self, kind):
+        return [t for t in self.tracks if t.kind == kind]
+
+    def select(self, kind, idx):
+        """The reference's Demuxer._select_stream (demux.py:335-355): kind is 'audio', 'subtitles' or 'video'."""
+        return select_stream(self.streams(kind), kind, idx, self.path)
+
+
 def select_stream(streams, kind, idx, path):
     """The reference's Demuxer._select_stream (demux.py:335-355) over a container's streams of one kind (objects with
     .id, .title, .info and .default): `idx` a stream id, or None for the only stream, else the default one."""

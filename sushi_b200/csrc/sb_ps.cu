@@ -4,7 +4,7 @@
 // the previous chunk reached.
 //   sb_ps_feed     one chunk: the carried bytes and the chunk side by side on the device, then
 //                    k_ps_mark      per 16 positions: the start codes there (00 00 01 xx, xx >= 0xB9); per-CTA counts
-//                    k_ps_offsets   one CTA: exclusive scan of the counts, the candidate total
+//                    k_scan_totals  one CTA: exclusive scan of the counts, the candidate total (sb_demux.cuh)
 //                    k_ps_cands     the candidates' positions, in order
 //                  (the candidate count comes back to size the launches), then
 //                    k_ps_link      one thread per candidate: its packet's length and the candidate it links to (or how
@@ -13,61 +13,28 @@
 //                                   round, every candidate on the chain marks the one 2^r links on, and the links double
 //                    k_ps_pes       one thread per candidate on the chain: the chain's end (the next chunk's carry, or a
 //                                   refusal), the chosen stream's PES header, per-CTA payload totals
-//                    k_ps_totals    one CTA: their exclusive scan on top of the running totals
+//                    k_scan_totals  one CTA: their exclusive scan on top of the running totals
 //                    k_ps_place     the payload's place in the elementary stream; the PES table
 //                    k_ps_copy      one warp per PES: its payload into the elementary-stream buffer
 //                  and returns; the running totals and the carry position come back before the next chunk is placed
 //   sb_ps_finish   the carried bytes as the file's end (a last PES may be cut), then the elementary stream through
 //                  sb::mp2_decode, messages naming the PES that holds a frame's header
 // The per-packet rules are in sb_ps.cuh, shared with the CPU emulation of the tests.
-#include "sb_decode.h"
+#include "sb_demux.cuh"
 #include "sb_ps.cuh"
-#include <algorithm>
+#include <memory>
 #include <new>
-#include <vector>
 
 using namespace sb;
 
 namespace {
 
-constexpr int kThreads = 256;
 constexpr int kPer = 16;                               // positions one k_ps_mark thread checks
-constexpr unsigned long long kNoError = ~0ull;
 
 struct Run { long long bytes, pes, carry; };           // payload bytes and PES so far; where the last chunk's carry starts
 struct PesRec { int64_t file_off, es_off; };           // one PES of the stream: its file offset, its payload's place
 struct Sel { int64_t off, len, dst; };                 // one chain packet's payload in the buffer (len 0: none kept)
                                                        // and its place in the elementary stream
-
-__device__ __forceinline__ void fail_at(unsigned long long* err, int64_t file_off, int code) {
-    atomicMin(err, ((unsigned long long)file_off << 8) | (unsigned)code);
-}
-
-// exclusive prefix of v over the CTA, *total the CTA's sum (every thread of the CTA calls it)
-__device__ long long block_exclusive(long long v, long long* total) {
-    __shared__ long long warp_sums[32];
-    const int lane = threadIdx.x & 31, w = threadIdx.x >> 5, nw = (blockDim.x + 31) >> 5;
-    long long x = v;
-    for (int o = 1; o < 32; o <<= 1) {
-        const long long y = __shfl_up_sync(0xFFFFFFFFu, x, o);
-        if (lane >= o) x += y;
-    }
-    if (lane == 31) warp_sums[w] = x;
-    __syncthreads();
-    if (w == 0) {
-        long long s = lane < nw ? warp_sums[lane] : 0;
-        for (int o = 1; o < 32; o <<= 1) {
-            const long long y = __shfl_up_sync(0xFFFFFFFFu, s, o);
-            if (lane >= o) s += y;
-        }
-        if (lane < nw) warp_sums[lane] = s;
-    }
-    __syncthreads();
-    const long long before = (w > 0 ? warp_sums[w - 1] : 0) + x - v;
-    *total = warp_sums[nw - 1];
-    __syncthreads();
-    return before;
-}
 
 // the start codes among positions [i0, i0 + kPer) below limit, as a bit mask
 __device__ __forceinline__ unsigned start_mask(const uint8_t* __restrict__ buf, int64_t i0, int64_t limit) {
@@ -86,19 +53,6 @@ k_ps_mark(const uint8_t* __restrict__ buf, int64_t limit, long long* __restrict_
     long long total;
     block_exclusive(__popc(start_mask(buf, i0, limit)), &total);
     if (threadIdx.x == 0) cta[blockIdx.x] = total;
-}
-
-__global__ void __launch_bounds__(1024)
-k_ps_offsets(long long* __restrict__ cta, int64_t n_cta, long long* __restrict__ count) {
-    long long base = 0;
-    for (int64_t t0 = 0; t0 < n_cta; t0 += blockDim.x) {
-        const int64_t t = t0 + threadIdx.x;
-        long long total;
-        const long long ex = block_exclusive(t < n_cta ? cta[t] : 0, &total);
-        if (t < n_cta) cta[t] = base + ex;
-        base += total;
-    }
-    if (threadIdx.x == 0) *count = base;
 }
 
 __global__ void __launch_bounds__(kThreads)
@@ -187,21 +141,6 @@ k_ps_pes(const uint8_t* __restrict__ buf, int64_t n, int at_end, int64_t file_of
     if (threadIdx.x == 0) { cta[2 * blockIdx.x] = tb; cta[2 * blockIdx.x + 1] = tp; }
 }
 
-__global__ void __launch_bounds__(1024)
-k_ps_totals(long long* __restrict__ cta, int64_t n_cta, Run* __restrict__ run) {
-    long long bytes = run->bytes, pes = run->pes;
-    for (int64_t t0 = 0; t0 < n_cta; t0 += blockDim.x) {
-        const int64_t t = t0 + threadIdx.x;
-        long long tb, tp;
-        const long long eb = block_exclusive(t < n_cta ? cta[2 * t] : 0, &tb);
-        const long long ep = block_exclusive(t < n_cta ? cta[2 * t + 1] : 0, &tp);
-        if (t < n_cta) { cta[2 * t] = bytes + eb; cta[2 * t + 1] = pes + ep; }
-        bytes += tb; pes += tp;
-    }
-    __syncthreads();
-    if (threadIdx.x == 0) { run->bytes = bytes; run->pes = pes; }
-}
-
 __global__ void __launch_bounds__(kThreads)
 k_ps_place(int64_t file_off0, const int64_t* __restrict__ pos, int64_t m, Sel* __restrict__ sel,
            const long long* __restrict__ cta, PesRec* __restrict__ tab) {
@@ -223,30 +162,13 @@ k_ps_copy(const uint8_t* __restrict__ buf, int64_t m, const Sel* __restrict__ se
     for (int64_t b = threadIdx.x & 31; b < s.len; b += 32) es[s.dst + b] = buf[s.off + b];
 }
 
-template <class T>
-int grow(T** p, int64_t* cap, int64_t used, int64_t need, cudaStream_t st) {
-    if (need <= *cap) return SB_OK;
-    const int64_t n = std::max(need, *cap + *cap / 2);
-    T* q = nullptr;
-    if (pool_alloc((void**)&q, sizeof(T) * (size_t)n + 16) != SB_OK) return SB_ENOMEM;
-    if (used > 0 && cudaMemcpyAsync(q, *p, sizeof(T) * (size_t)used, cudaMemcpyDeviceToDevice, st) != cudaSuccess) {
-        pool_free(q);
-        return SB_ECUDA;
-    }
-    pool_free(*p);
-    *p = q;
-    *cap = n;
-    return SB_OK;
-}
-
 }  // namespace
 
-struct sb_ps {
+struct sb_ps : ChunkedDemux<Run> {
     int stream_id = 0;
     uint8_t* d_buf[2] = {nullptr, nullptr}; int64_t buf_cap[2] = {0, 0};
     int cur = 0;                                        // the buffer the last chunk went to
     int64_t buf_len = 0, buf_off = 0;                   // its bytes, and the file offset of its first byte
-    int64_t next_offset = 0;
     long long* d_cta = nullptr; int64_t cta_cap = 0;
     int64_t* d_pos = nullptr; int64_t pos_cap = 0;
     sbps::Link* d_links = nullptr; int64_t links_cap = 0;
@@ -258,12 +180,13 @@ struct sb_ps {
     Run* d_run = nullptr;
     long long* d_count = nullptr;
     uint32_t* d_cut = nullptr;
-    unsigned long long* d_err = nullptr;
-    Run* h_run = nullptr;                               // pinned copy of *d_run
-    long long* h_count = nullptr;                       // pinned copy of *d_count
-    cudaEvent_t done = nullptr;
-    bool pending = false, finished = false;
+    long long* h_count = nullptr;                       // pinned copy of *d_count; *h_run is that of *d_run
 
+    ~sb_ps() {
+        release_demux();
+        pool_free(d_run); pool_free(d_count); pool_free(d_cut);
+        if (h_count) cudaFreeHost(h_count);
+    }
     void release_demux() {
         for (int b = 0; b < 2; ++b) { pool_free(d_buf[b]); pool_free(d_jump[b]); d_buf[b] = nullptr; d_jump[b] = nullptr;
                                       buf_cap[b] = jump_cap[b] = 0; }
@@ -276,14 +199,6 @@ struct sb_ps {
 };
 
 namespace {
-
-// Wait for the kernels of the last chunk: the running totals and the carry position are then in *h_run
-int settle(sb_ps* t, const char* who) {
-    if (!t->pending) return SB_OK;
-    SB_TRY(cuda_result(cudaEventSynchronize(t->done), who));
-    t->pending = false;
-    return SB_OK;
-}
 
 // Scan buf[0, n) of the current buffer (file offset base): the packet chain from position 0, the stream's payload
 // appended.  `at_end`: the buffer ends the file.  Returns once the kernels are enqueued (the candidate count having
@@ -300,7 +215,7 @@ int scan_buffer(sb_ps* t, const uint8_t* buf, int64_t n, int64_t base, bool at_e
     {
         ProfScope ps("ps_mark", 3);
         k_ps_mark<<<(unsigned)n_cta, kThreads, 0, c.stream>>>(buf, limit, t->d_cta);
-        k_ps_offsets<<<1, 1024, 0, c.stream>>>(t->d_cta, n_cta, t->d_count);
+        k_scan_totals<1><<<1, 1024, 0, c.stream>>>(t->d_cta, n_cta, nullptr, t->d_count);
         k_ps_cands<<<(unsigned)n_cta, kThreads, 0, c.stream>>>(buf, limit, t->d_cta, t->d_pos);
         e = cudaGetLastError();
     }
@@ -335,7 +250,8 @@ int scan_buffer(sb_ps* t, const uint8_t* buf, int64_t n, int64_t base, bool at_e
         ProfScope ps("ps_compact", 4);
         k_ps_pes<<<(unsigned)m_cta, kThreads, 0, c.stream>>>(buf, n, at_end, base, t->stream_id, t->d_pos, m, t->d_links,
                                                             t->d_on, t->d_sel, t->d_cta, t->d_run, t->d_cut, t->d_err);
-        k_ps_totals<<<1, 1024, 0, c.stream>>>(t->d_cta, m_cta, t->d_run);
+        k_scan_totals<2><<<1, 1024, 0, c.stream>>>(t->d_cta, m_cta, reinterpret_cast<long long*>(t->d_run),
+                                                  reinterpret_cast<long long*>(t->d_run));
         k_ps_place<<<(unsigned)m_cta, kThreads, 0, c.stream>>>(base, t->d_pos, m, t->d_sel, t->d_cta, t->d_tab);
         k_ps_copy<<<(unsigned)((m * 32 + kThreads - 1) / kThreads + 1), kThreads, 0, c.stream>>>(buf, m, t->d_sel, t->d_es);
         e = cudaGetLastError();
@@ -352,44 +268,34 @@ int scan_buffer(sb_ps* t, const uint8_t* buf, int64_t n, int64_t base, bool at_e
 extern "C" {
 
 int sb_ps_open(int32_t stream_id, int32_t substream_id, sb_ps** out) {
+    const char* who = "sb_ps_open";
     Ctx& c = ctx();
-    if (!c.inited) SB_FAIL(SB_ESTATE, "sb_ps_open: library not initialised (call sb_init)");
-    if (!out) SB_FAIL(SB_EINVAL, "sb_ps_open: NULL argument");
+    SB_TRY(entry_check(who, out));
     if (stream_id < 0xC0 || stream_id > 0xDF)
         SB_FAIL(SB_EINVAL, "sb_ps_open: stream id 0x%x (MPEG audio streams, 0xC0 to 0xDF, are decoded)", stream_id);
     if (substream_id != -1) SB_FAIL(SB_EINVAL, "sb_ps_open: substream %d (MPEG audio streams have none)", substream_id);
-    sb_ps* t = new (std::nothrow) sb_ps();
+    std::unique_ptr<sb_ps> t(new (std::nothrow) sb_ps());
     if (!t) SB_FAIL(SB_ENOMEM, "sb_ps_open: out of host memory");
     t->stream_id = stream_id;
-    cudaError_t e = cudaMallocHost((void**)&t->h_run, sizeof(Run));
-    if (e == cudaSuccess) e = cudaMallocHost((void**)&t->h_count, sizeof(long long));
-    if (e == cudaSuccess) e = cudaEventCreateWithFlags(&t->done, cudaEventDisableTiming);
-    if (e == cudaSuccess) *t->h_run = Run{0, 0, 0};
-    if (e != cudaSuccess) { sb_ps_destroy(t); SB_FAIL(SB_ECUDA, "sb_ps_open: %s", cudaGetErrorString(e)); }
+    SB_TRY(t->open(who));
+    SB_TRY(cuda_result(cudaMallocHost((void**)&t->h_count, sizeof(long long)), who));
     if (pool_alloc((void**)&t->d_run, sizeof(Run)) != SB_OK || pool_alloc((void**)&t->d_count, 16) != SB_OK ||
-        pool_alloc((void**)&t->d_cut, 16) != SB_OK || pool_alloc((void**)&t->d_err, 16) != SB_OK) {
-        sb_ps_destroy(t);
+        pool_alloc((void**)&t->d_cut, 16) != SB_OK)
         SB_FAIL(SB_ENOMEM, "sb_ps_open: out of device memory");
-    }
-    e = cudaMemsetAsync(t->d_run, 0, sizeof(Run), c.stream);
+    cudaError_t e = cudaMemsetAsync(t->d_run, 0, sizeof(Run), c.stream);
     if (e == cudaSuccess) e = cudaMemsetAsync(t->d_cut, 0, sizeof(uint32_t), c.stream);
-    if (e == cudaSuccess) e = cudaMemsetAsync(t->d_err, 0xFF, sizeof(unsigned long long), c.stream);
-    if (e != cudaSuccess) { sb_ps_destroy(t); SB_FAIL(SB_ECUDA, "sb_ps_open: %s", cudaGetErrorString(e)); }
-    *out = t;
+    SB_TRY(cuda_result(e, who));
+    *out = t.release();
     return SB_OK;
 }
 
 int sb_ps_feed(sb_ps* t, const void* host_chunk, int64_t nbytes, int64_t file_offset) {
     const char* who = "sb_ps_feed";
     Ctx& c = ctx();
-    if (!c.inited) SB_FAIL(SB_ESTATE, "sb_ps_feed: library not initialised (call sb_init)");
-    if (!t || (!host_chunk && nbytes)) SB_FAIL(SB_EINVAL, "sb_ps_feed: NULL argument");
-    if (t->finished) SB_FAIL(SB_ESTATE, "sb_ps_feed: the stream is finished");
-    if (nbytes < 0) SB_FAIL(SB_EINVAL, "sb_ps_feed: %lld bytes", (long long)nbytes);
-    if (file_offset != t->next_offset) SB_FAIL(SB_EINVAL, "sb_ps_feed: chunk at byte offset %lld, expected %lld",
-                                               (long long)file_offset, (long long)t->next_offset);
+    SB_TRY(entry_check(who, t && (host_chunk || !nbytes)));
+    SB_TRY(t->feed_check(who, nbytes, file_offset, 1));
     if (!nbytes) return SB_OK;
-    SB_TRY(settle(t, who));
+    SB_TRY(t->settle(who));
     // the bytes from the chain position the last chunk reached, then this chunk, in the other buffer
     const int64_t carry_from = t->buf_len ? std::min<int64_t>(t->h_run->carry, t->buf_len) : 0;
     const int64_t carry = t->buf_len - carry_from, n = carry + nbytes;
@@ -418,26 +324,20 @@ int sb_ps_finish(sb_ps* t, int32_t* cut, sb_pcm** out) {
     const char* who = "sb_ps_finish";
     Ctx& c = ctx();
     SB_TRY(entry_check(who, t && cut && out));
-    if (t->finished) SB_FAIL(SB_ESTATE, "sb_ps_finish: the stream is finished");
-    t->finished = true;
-    struct ReleaseDemux { sb_ps* t; ~ReleaseDemux() { t->release_demux(); } } release_demux{t};
-    SB_TRY(settle(t, who));
+    SB_TRY(t->finish_check(who));
+    ReleaseDemux<sb_ps> release_demux{t};
+    SB_TRY(t->settle(who));
     // what the last chunk left over, as the end of the file; fewer than 4 bytes cannot start a packet (a file cut
     // inside a start code)
     const int64_t carry_from = t->buf_len ? std::min<int64_t>(t->h_run->carry, t->buf_len) : 0;
     if (t->buf_len - carry_from >= 4) {
         SB_TRY(scan_buffer(t, t->d_buf[t->cur] + carry_from, t->buf_len - carry_from, t->buf_off + carry_from, true, who));
-        SB_TRY(settle(t, who));
+        SB_TRY(t->settle(who));
     }
-    unsigned long long err = kNoError;
+    SB_TRY(t->check_failure(who, [](int k) { return k == sbps::kBadPesHeader ? "PES packet" : "program stream packet"; },
+                            sbps::error_text));
     uint32_t was_cut = 0;
-    SB_TRY(collect(cudaSuccess, &err, t->d_err, 1, who));
     SB_TRY(collect(cudaSuccess, &was_cut, t->d_cut, 1, who));
-    if (err != kNoError) {
-        const int k = (int)(err & 0xFF);
-        SB_FAIL(SB_EINVAL, "%s at byte offset %lld: %s", k == sbps::kBadPesHeader ? "PES packet" : "program stream packet",
-                (long long)(err >> 8), sbps::error_text(k));
-    }
     const Run run = *t->h_run;
     if (run.pes < 1 || run.bytes < 1) SB_FAIL(SB_EINVAL, "stream 0x%x carries no PES payload", t->stream_id);
     std::vector<uint8_t> host((size_t)run.bytes + 1);
@@ -448,27 +348,13 @@ int sb_ps_finish(sb_ps* t, int32_t* cut, sb_pcm** out) {
                                               cudaMemcpyDeviceToHost, c.stream);
     SB_TRY(collect(e, host.data(), t->d_es, run.bytes, who));
     // messages name the PES holding a stream byte
-    auto where = [&](int64_t b) -> int64_t {
-        const int64_t k = std::upper_bound(tab.begin(), tab.end(), b, [](int64_t v, const PesRec& r) { return v < r.es_off; })
-                          - tab.begin() - 1;
-        return k >= 0 ? tab[(size_t)k].file_off : -1;
-    };
+    auto where = [&](int64_t b) { return file_offset_of(tab, b); };
     int32_t dropped = 0;
     SB_TRY(mp2_decode(host.data(), t->d_es, run.bytes, where, &dropped, out));
     *cut = was_cut || dropped;
     return SB_OK;
 }
 
-int sb_ps_destroy(sb_ps* t) {
-    if (!t) return SB_OK;
-    if (t->pending) cudaEventSynchronize(t->done);
-    t->release_demux();
-    pool_free(t->d_run); pool_free(t->d_count); pool_free(t->d_cut); pool_free(t->d_err);
-    if (t->h_run) cudaFreeHost(t->h_run);
-    if (t->h_count) cudaFreeHost(t->h_count);
-    if (t->done) cudaEventDestroy(t->done);
-    delete t;
-    return SB_OK;
-}
+int sb_ps_destroy(sb_ps* t) { return destroy_demux(t); }
 
 }  // extern "C"

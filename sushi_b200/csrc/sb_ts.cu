@@ -4,7 +4,7 @@
 //                    k_ts_scan      one thread per packet: the sync byte of every packet, the header and adaptation
 //                                   field of the PID's packets; per-CTA totals of the PID's payload bytes, packets and
 //                                   PES starts
-//                    k_ts_totals    one CTA: exclusive scan of the CTA totals on top of the running totals
+//                    k_scan_totals  one CTA: exclusive scan of the CTA totals on top of the running totals (sb_demux.cuh)
 //                    k_ts_scatter   the PID's payload bytes appended to the elementary-stream buffer, its packets to the
 //                                   packet table, its payload-unit starts to the PES table
 //                    k_ts_cc        one thread per appended packet: the continuity counter against the packet before
@@ -15,18 +15,14 @@
 //                  over sample frames into interleaved int16) or k_ts_gather + the TrueHD decoder of sb_truehd.cu, into
 //                  an sb_pcm
 // The per-packet and per-PES rules are in sb_ts.cuh, shared with the CPU emulation of the tests.
-#include "sb_decode.h"
+#include "sb_demux.cuh"
 #include "sb_ts.cuh"
-#include <algorithm>
+#include <memory>
 #include <new>
-#include <vector>
 
 using namespace sb;
 
 namespace {
-
-constexpr int kThreads = 256;
-constexpr unsigned long long kNoError = ~0ull;
 
 struct Totals { long long bytes, packets, pes; };    // the PID's payload bytes, packets and PES starts
 
@@ -37,45 +33,6 @@ struct PktRec {                                      // one packet of the PID
     uint8_t pusi, cc, disc, has_payload;
 };
 struct PesStart { int64_t es_off, pkt; };
-
-// first failure wins: the byte offset in the high bits, the code in the low 8
-__device__ __forceinline__ void fail_at(unsigned long long* err, int64_t file_off, int code) {
-    atomicMin(err, ((unsigned long long)file_off << 8) | (unsigned)code);
-}
-
-// exclusive prefix of v over the CTA, *total the CTA's sum (every thread of the CTA calls it)
-__device__ long long block_exclusive(long long v, long long* total) {
-    __shared__ long long warp_sums[32];
-    const int lane = threadIdx.x & 31, w = threadIdx.x >> 5, nw = (blockDim.x + 31) >> 5;
-    long long x = v;
-    for (int o = 1; o < 32; o <<= 1) {
-        const long long y = __shfl_up_sync(0xFFFFFFFFu, x, o);
-        if (lane >= o) x += y;
-    }
-    if (lane == 31) warp_sums[w] = x;
-    __syncthreads();
-    if (w == 0) {
-        long long s = lane < nw ? warp_sums[lane] : 0;
-        for (int o = 1; o < 32; o <<= 1) {
-            const long long y = __shfl_up_sync(0xFFFFFFFFu, s, o);
-            if (lane >= o) s += y;
-        }
-        if (lane < nw) warp_sums[lane] = s;
-    }
-    __syncthreads();
-    const long long before = (w > 0 ? warp_sums[w - 1] : 0) + x - v;
-    *total = warp_sums[nw - 1];
-    __syncthreads();                                  // warp_sums is reused by the next call
-    return before;
-}
-
-__device__ __forceinline__ Totals block_exclusive3(const Totals& v, Totals* total) {
-    Totals r;
-    r.bytes = block_exclusive(v.bytes, &total->bytes);
-    r.packets = block_exclusive(v.packets, &total->packets);
-    r.pes = block_exclusive(v.pes, &total->pes);
-    return r;
-}
 
 __device__ __forceinline__ Totals packet_counts(const sbts::Packet& q) {
     Totals t;
@@ -101,24 +58,12 @@ k_ts_scan(const uint8_t* __restrict__ chunk, int64_t n_pk, int psize, int pid, i
         else if (id == pid) q = r;
         info[i] = q;
     }
+    const Totals v = packet_counts(q);
     Totals total;
-    block_exclusive3(packet_counts(q), &total);
+    block_exclusive(v.bytes, &total.bytes);
+    block_exclusive(v.packets, &total.packets);
+    block_exclusive(v.pes, &total.pes);
     if (threadIdx.x == 0) cta[blockIdx.x] = total;
-}
-
-__global__ void __launch_bounds__(1024)
-k_ts_totals(Totals* __restrict__ cta, int64_t n_cta, Totals* __restrict__ run) {
-    Totals base = run[1];                              // after the previous chunk
-    if (threadIdx.x == 0) run[0] = base;
-    for (int64_t t0 = 0; t0 < n_cta; t0 += blockDim.x) {
-        const int64_t t = t0 + threadIdx.x;
-        Totals v = {0, 0, 0}, total;
-        if (t < n_cta) v = cta[t];
-        const Totals ex = block_exclusive3(v, &total);
-        if (t < n_cta) cta[t] = Totals{base.bytes + ex.bytes, base.packets + ex.packets, base.pes + ex.pes};
-        base.bytes += total.bytes; base.packets += total.packets; base.pes += total.pes;
-    }
-    if (threadIdx.x == 0) run[1] = base;
 }
 
 __global__ void __launch_bounds__(kThreads)
@@ -131,7 +76,10 @@ k_ts_scatter(const uint8_t* __restrict__ chunk, int64_t n_pk, int psize, int64_t
     if (i < n_pk) q = info[i];
     Totals total;
     const Totals v = packet_counts(q);
-    Totals at = block_exclusive3(v, &total);
+    Totals at;
+    at.bytes = block_exclusive(v.bytes, &total.bytes);
+    at.packets = block_exclusive(v.packets, &total.packets);
+    at.pes = block_exclusive(v.pes, &total.pes);
     if (!v.packets) return;
     const Totals base = cta[blockIdx.x];
     at.bytes += base.bytes; at.packets += base.packets; at.pes += base.pes;
@@ -147,9 +95,10 @@ k_ts_scatter(const uint8_t* __restrict__ chunk, int64_t n_pk, int psize, int64_t
 }
 
 __global__ void __launch_bounds__(kThreads)
-k_ts_cc(const PktRec* __restrict__ tab, const Totals* __restrict__ run, unsigned long long* __restrict__ err) {
-    const int64_t j = run[0].packets + (int64_t)blockIdx.x * blockDim.x + threadIdx.x;
-    if (j >= run[1].packets || j == 0) return;
+k_ts_cc(const PktRec* __restrict__ tab, int64_t first, const Totals* __restrict__ run,
+        unsigned long long* __restrict__ err) {
+    const int64_t j = first + (int64_t)blockIdx.x * blockDim.x + threadIdx.x;
+    if (j >= run->packets || j == 0) return;
     const PktRec a = tab[j - 1], b = tab[j];
     sbts::Packet q;
     q.cc = b.cc; q.disc = b.disc; q.has_payload = b.has_payload;
@@ -199,36 +148,6 @@ k_pes_index(const uint8_t* __restrict__ es, int64_t es_total, const PesStart* __
     count[s] = sbts::lpcm_frames(p.payload_len, f);
 }
 
-// exclusive scan of n int64 values in place: tile sums, one CTA over the tiles, then each tile
-__global__ void __launch_bounds__(kThreads)
-k_scan_tiles(const int64_t* __restrict__ v, int64_t n, long long* __restrict__ tiles) {
-    const int64_t i = (int64_t)blockIdx.x * blockDim.x + threadIdx.x;
-    long long total;
-    block_exclusive(i < n ? v[i] : 0, &total);
-    if (threadIdx.x == 0) tiles[blockIdx.x] = total;
-}
-
-__global__ void __launch_bounds__(1024)
-k_scan_top(long long* __restrict__ tiles, int64_t n_tiles, long long* __restrict__ total_out) {
-    long long base = 0;
-    for (int64_t t0 = 0; t0 < n_tiles; t0 += blockDim.x) {
-        const int64_t t = t0 + threadIdx.x;
-        long long total;
-        const long long ex = block_exclusive(t < n_tiles ? tiles[t] : 0, &total);
-        if (t < n_tiles) tiles[t] = base + ex;
-        base += total;
-    }
-    if (threadIdx.x == 0) *total_out = base;
-}
-
-__global__ void __launch_bounds__(kThreads)
-k_scan_apply(int64_t* __restrict__ v, int64_t n, const long long* __restrict__ tiles) {
-    const int64_t i = (int64_t)blockIdx.x * blockDim.x + threadIdx.x;
-    long long total;
-    const long long ex = block_exclusive(i < n ? v[i] : 0, &total);
-    if (i < n) v[i] = tiles[blockIdx.x] + ex;
-}
-
 __global__ void __launch_bounds__(kThreads)
 k_bdlpcm_decode(const uint8_t* __restrict__ es, const int64_t* __restrict__ off, const int64_t* __restrict__ start,
                 int64_t n_pes, int64_t frames, sbts::Lpcm f, int16_t* __restrict__ pcm) {
@@ -250,39 +169,24 @@ k_ts_gather(const uint8_t* __restrict__ es, const int64_t* __restrict__ off, con
     for (int64_t b = threadIdx.x; b < len[s]; b += blockDim.x) dst[b] = src[b];
 }
 
-template <class T>
-int grow(T** p, int64_t* cap, int64_t used, int64_t need, cudaStream_t st) {
-    if (need <= *cap) return SB_OK;
-    const int64_t n = std::max(need, *cap + *cap / 2);
-    T* q = nullptr;
-    if (pool_alloc((void**)&q, sizeof(T) * (size_t)n + 16) != SB_OK) return SB_ENOMEM;
-    if (used > 0 && cudaMemcpyAsync(q, *p, sizeof(T) * (size_t)used, cudaMemcpyDeviceToDevice, st) != cudaSuccess) {
-        pool_free(q);
-        return SB_ECUDA;
-    }
-    pool_free(*p);
-    *p = q;
-    *cap = n;
-    return SB_OK;
-}
-
 }  // namespace
 
-struct sb_ts {
+struct sb_ts : ChunkedDemux<Totals> {
     int psize = 188, pid = 0, codec = 0;
-    int64_t next_offset = 0;
     uint8_t* d_chunk = nullptr; int64_t chunk_cap = 0;
     sbts::Packet* d_info = nullptr; int64_t info_cap = 0;
     Totals* d_cta = nullptr; int64_t cta_cap = 0;
     uint8_t* d_es = nullptr; int64_t es_cap = 0;
     PktRec* d_tab = nullptr; int64_t tab_cap = 0;
     PesStart* d_pes = nullptr; int64_t pes_cap = 0;
-    Totals* d_run = nullptr;                            // [0] before the last chunk, [1] after it
-    unsigned long long* d_err = nullptr;
-    Totals* h_run = nullptr;                            // pinned copy of d_run[1]
-    cudaEvent_t done = nullptr, copied = nullptr;
-    bool pending = false, finished = false;
+    Totals* d_run = nullptr;                            // after the last chunk; *h_run is its pinned copy
+    cudaEvent_t copied = nullptr;
 
+    ~sb_ts() {
+        release_demux();
+        pool_free(d_run);
+        if (copied) cudaEventDestroy(copied);
+    }
     void release_demux() {
         pool_free(d_chunk); pool_free(d_info); pool_free(d_cta); pool_free(d_es); pool_free(d_tab); pool_free(d_pes);
         d_chunk = nullptr; d_info = nullptr; d_cta = nullptr; d_es = nullptr; d_tab = nullptr; d_pes = nullptr;
@@ -293,48 +197,32 @@ struct sb_ts {
 extern "C" {
 
 int sb_ts_open(int packet_size, int32_t pid, int32_t codec, sb_ts** out) {
+    const char* who = "sb_ts_open";
     Ctx& c = ctx();
-    if (!c.inited) SB_FAIL(SB_ESTATE, "sb_ts_open: library not initialised (call sb_init)");
-    if (!out) SB_FAIL(SB_EINVAL, "sb_ts_open: NULL argument");
+    SB_TRY(entry_check(who, out));
     if (packet_size != 188 && packet_size != 192) SB_FAIL(SB_EINVAL, "sb_ts_open: packet size %d (188 or 192)", packet_size);
     if (pid < 0 || pid > 0x1FFE) SB_FAIL(SB_EINVAL, "sb_ts_open: PID %d", pid);
     if (codec != SB_TS_PCM_BLURAY && codec != SB_TS_TRUEHD && codec != SB_TS_MP2) SB_FAIL(SB_EINVAL, "sb_ts_open: codec %d", codec);
-    sb_ts* t = new (std::nothrow) sb_ts();
+    std::unique_ptr<sb_ts> t(new (std::nothrow) sb_ts());
     if (!t) SB_FAIL(SB_ENOMEM, "sb_ts_open: out of host memory");
     t->psize = packet_size; t->pid = pid; t->codec = codec;
-    cudaError_t e = cudaMallocHost((void**)&t->h_run, sizeof(Totals));
-    if (e == cudaSuccess) e = cudaEventCreateWithFlags(&t->done, cudaEventDisableTiming);
-    if (e == cudaSuccess) e = cudaEventCreateWithFlags(&t->copied, cudaEventDisableTiming);
-    if (e == cudaSuccess) *t->h_run = Totals{0, 0, 0};
-    if (e != cudaSuccess) { sb_ts_destroy(t); SB_FAIL(SB_ECUDA, "sb_ts_open: %s", cudaGetErrorString(e)); }
-    if (pool_alloc((void**)&t->d_run, 2 * sizeof(Totals)) != SB_OK || pool_alloc((void**)&t->d_err, 16) != SB_OK) {
-        sb_ts_destroy(t);
-        SB_FAIL(SB_ENOMEM, "sb_ts_open: out of device memory");
-    }
-    e = cudaMemsetAsync(t->d_run, 0, 2 * sizeof(Totals), c.stream);
-    if (e == cudaSuccess) e = cudaMemsetAsync(t->d_err, 0xFF, sizeof(unsigned long long), c.stream);
-    if (e != cudaSuccess) { sb_ts_destroy(t); SB_FAIL(SB_ECUDA, "sb_ts_open: %s", cudaGetErrorString(e)); }
-    *out = t;
+    SB_TRY(t->open(who));
+    SB_TRY(cuda_result(cudaEventCreateWithFlags(&t->copied, cudaEventDisableTiming), who));
+    if (pool_alloc((void**)&t->d_run, sizeof(Totals)) != SB_OK) SB_FAIL(SB_ENOMEM, "sb_ts_open: out of device memory");
+    SB_TRY(cuda_result(cudaMemsetAsync(t->d_run, 0, sizeof(Totals), c.stream), who));
+    *out = t.release();
     return SB_OK;
 }
 
 int sb_ts_feed(sb_ts* t, const void* host_chunk, int64_t nbytes, int64_t file_offset) {
+    const char* who = "sb_ts_feed";
     Ctx& c = ctx();
-    if (!c.inited) SB_FAIL(SB_ESTATE, "sb_ts_feed: library not initialised (call sb_init)");
-    if (!t || (!host_chunk && nbytes)) SB_FAIL(SB_EINVAL, "sb_ts_feed: NULL argument");
-    if (t->finished) SB_FAIL(SB_ESTATE, "sb_ts_feed: the stream is finished");
-    if (nbytes < 0 || nbytes % t->psize) SB_FAIL(SB_EINVAL, "sb_ts_feed: %lld bytes is not a whole number of %d-byte packets",
-                                                 (long long)nbytes, t->psize);
-    if (file_offset != t->next_offset) SB_FAIL(SB_EINVAL, "sb_ts_feed: chunk at byte offset %lld, expected %lld",
-                                               (long long)file_offset, (long long)t->next_offset);
+    SB_TRY(entry_check(who, t && (host_chunk || !nbytes)));
+    SB_TRY(t->feed_check(who, nbytes, file_offset, t->psize));
     if (!nbytes) return SB_OK;
     const int64_t n_pk = nbytes / t->psize, n_cta = (n_pk + kThreads - 1) / kThreads;
     // the totals after the previous chunk: they place this one
-    if (t->pending) {
-        const cudaError_t e = cudaEventSynchronize(t->done);
-        if (e != cudaSuccess) SB_FAIL(SB_ECUDA, "sb_ts_feed: %s", cudaGetErrorString(e));
-        t->pending = false;
-    }
+    SB_TRY(t->settle(who));
     const Totals run = *t->h_run;
     int rc = grow(&t->d_chunk, &t->chunk_cap, 0, nbytes, c.stream);
     if (rc == SB_OK) rc = grow(&t->d_info, &t->info_cap, 0, n_pk, c.stream);
@@ -353,76 +241,37 @@ int sb_ts_feed(sb_ts* t, const void* host_chunk, int64_t nbytes, int64_t file_of
     }
     if (e == cudaSuccess) {
         ProfScope ps("ts_compact", 2);
-        k_ts_totals<<<1, 1024, 0, c.stream>>>(t->d_cta, n_cta, t->d_run);
+        long long* run_d = reinterpret_cast<long long*>(t->d_run);
+        k_scan_totals<3><<<1, 1024, 0, c.stream>>>(reinterpret_cast<long long*>(t->d_cta), n_cta, run_d, run_d);
         k_ts_scatter<<<(unsigned)n_cta, kThreads, 0, c.stream>>>(t->d_chunk, n_pk, t->psize, file_offset, t->d_info,
                                                                  t->d_cta, t->d_es, t->d_tab, t->d_pes);
         e = cudaGetLastError();
     }
     if (e == cudaSuccess) {
         ProfScope ps("ts_scan");
-        k_ts_cc<<<(unsigned)n_cta, kThreads, 0, c.stream>>>(t->d_tab, t->d_run, t->d_err);
+        k_ts_cc<<<(unsigned)n_cta, kThreads, 0, c.stream>>>(t->d_tab, run.packets, t->d_run, t->d_err);
         e = cudaGetLastError();
     }
-    if (e == cudaSuccess) e = cudaMemcpyAsync(t->h_run, t->d_run + 1, sizeof(Totals), cudaMemcpyDeviceToHost, c.stream);
+    if (e == cudaSuccess) e = cudaMemcpyAsync(t->h_run, t->d_run, sizeof(Totals), cudaMemcpyDeviceToHost, c.stream);
     if (e == cudaSuccess) e = cudaEventRecord(t->done, c.stream);
-    if (e != cudaSuccess) SB_FAIL(SB_ECUDA, "sb_ts_feed: %s", cudaGetErrorString(e));
+    SB_TRY(cuda_result(e, who));
     t->pending = true;
     t->next_offset += nbytes;
     // the caller may refill its buffer once the copy has run; the kernels go on behind it
-    e = cudaEventSynchronize(t->copied);
-    if (e != cudaSuccess) SB_FAIL(SB_ECUDA, "sb_ts_feed: %s", cudaGetErrorString(e));
-    return SB_OK;
+    return cuda_result(cudaEventSynchronize(t->copied), who);
 }
-
-}  // extern "C"
-
-namespace {
-
-// exclusive scan of d_v[0..n) in place on the library stream; the sum comes back in *total
-int scan_i64(int64_t* d_v, int64_t n, int64_t* total) {
-    Ctx& c = ctx();
-    const int64_t tiles = (n + kThreads - 1) / kThreads;
-    long long* d_tiles = nullptr;
-    if (pool_alloc((void**)&d_tiles, sizeof(long long) * (size_t)(tiles + 1)) != SB_OK) SB_FAIL(SB_ENOMEM, "sb_ts_finish: out of device memory");
-    cudaError_t e = cudaSuccess;
-    {
-        ProfScope ps("pes_index", 3);
-        k_scan_tiles<<<(unsigned)tiles, kThreads, 0, c.stream>>>(d_v, n, d_tiles);
-        k_scan_top<<<1, 1024, 0, c.stream>>>(d_tiles, tiles, d_tiles + tiles);
-        k_scan_apply<<<(unsigned)tiles, kThreads, 0, c.stream>>>(d_v, n, d_tiles);
-        e = cudaGetLastError();
-    }
-    long long t = 0;
-    if (e == cudaSuccess) e = cudaMemcpyAsync(&t, d_tiles + tiles, sizeof(t), cudaMemcpyDeviceToHost, c.stream);
-    if (e == cudaSuccess) e = cudaStreamSynchronize(c.stream);
-    pool_free(d_tiles);
-    if (e != cudaSuccess) SB_FAIL(SB_ECUDA, "sb_ts_finish: %s", cudaGetErrorString(e));
-    *total = t;
-    return SB_OK;
-}
-
-}  // namespace
-
-extern "C" {
 
 int sb_ts_finish(sb_ts* t, int32_t* cut, sb_pcm** out) {
     const char* who = "sb_ts_finish";
     Ctx& c = ctx();
     SB_TRY(entry_check(who, t && cut && out));
-    if (t->finished) SB_FAIL(SB_ESTATE, "sb_ts_finish: the stream is finished");
-    t->finished = true;
+    SB_TRY(t->finish_check(who));
     // the demultiplexer's buffers go when this returns, on whichever line: after truehd_index_device, whose `where`
     // reads t->d_tab when it words a message
-    struct ReleaseDemux { sb_ts* t; ~ReleaseDemux() { t->release_demux(); } } release_demux{t};
-    unsigned long long err = kNoError;
-    SB_TRY(collect(cudaSuccess, &err, t->d_err, 1, who));
+    ReleaseDemux<sb_ts> release_demux{t};
+    auto noun = [](int k) { return k <= sbts::kCcGap ? "transport stream packet" : "PES packet"; };
+    SB_TRY(t->check_failure(who, noun, sbts::error_text));
     const Totals run = *t->h_run;
-    auto refuse = [&](unsigned long long code) {
-        const int k = (int)(code & 0xFF);
-        SB_FAIL(SB_EINVAL, "%s at byte offset %lld: %s", k <= sbts::kCcGap ? "transport stream packet" : "PES packet",
-                (long long)(code >> 8), sbts::error_text(k));
-    };
-    if (err != kNoError) return refuse(err);
     if (run.pes < 1) SB_FAIL(SB_EINVAL, "PID %d carries no PES packet", t->pid);
     const int64_t n_pes = run.pes;
     Blocks blocks;
@@ -440,12 +289,11 @@ int sb_ts_finish(sb_ts* t, int32_t* cut, sb_pcm** out) {
             t->d_es, run.bytes, t->d_pes, n_pes, t->d_tab, t->codec, d_off, d_count, d_misc, t->d_err);
         e = cudaGetLastError();
     }
-    if (e == cudaSuccess) e = cudaMemcpyAsync(&err, t->d_err, sizeof(err), cudaMemcpyDeviceToHost, c.stream);
     SB_TRY(collect(e, misc, d_misc, 2, who));
-    if (err != kNoError) return refuse(err);
+    SB_TRY(t->check_failure(who, noun, sbts::error_text));
     // per PES: the first sample frame (LPCM) or the first byte of the TrueHD stream (TrueHD)
     int64_t total = 0;
-    SB_TRY(scan_i64(d_count, n_pes, &total));
+    SB_TRY(scan_i64(d_count, n_pes, &total, "pes_index", who));
     *cut = misc[1] ? 1 : 0;
     if (t->codec == SB_TS_PCM_BLURAY) {
         sbts::Lpcm f;
@@ -502,9 +350,7 @@ int sb_ts_finish(sb_ts* t, int32_t* cut, sb_pcm** out) {
             if (cudaMemcpy(tab.data(), t->d_tab, sizeof(PktRec) * (size_t)run.packets, cudaMemcpyDeviceToHost) != cudaSuccess)
                 return -1;
         }
-        const int64_t k = std::upper_bound(tab.begin(), tab.end(), es, [](int64_t v, const PktRec& r) { return v < r.es_off; })
-                          - tab.begin() - 1;
-        return k >= 0 ? tab[(size_t)k].file_off : -1;
+        return file_offset_of(tab, es);
     };
     if (t->codec == SB_TS_MP2) {
         int32_t dropped = 0;
@@ -516,16 +362,6 @@ int sb_ts_finish(sb_ts* t, int32_t* cut, sb_pcm** out) {
     return truehd_index_device(host.data(), d_thd, total, &zero, d_block, 1, where, out);
 }
 
-int sb_ts_destroy(sb_ts* t) {
-    if (!t) return SB_OK;
-    if (t->pending) cudaEventSynchronize(t->done);
-    t->release_demux();
-    pool_free(t->d_run); pool_free(t->d_err);
-    if (t->h_run) cudaFreeHost(t->h_run);
-    if (t->done) cudaEventDestroy(t->done);
-    if (t->copied) cudaEventDestroy(t->copied);
-    delete t;
-    return SB_OK;
-}
+int sb_ts_destroy(sb_ts* t) { return destroy_demux(t); }
 
 }  // extern "C"

@@ -25,7 +25,7 @@ import zlib
 import numpy as np
 
 from . import _native, alac, flac, swr, truehd, tta, wavpack
-from .common import Audio, SushiError, py2_round, select_stream
+from .common import Audio, Container, SushiError, py2_round
 
 MATROSKA_EXTENSIONS = ('.mkv', '.mka', '.mks', '.webm')
 EBML_MAGIC = b'\x1a\x45\xdf\xa3'
@@ -247,7 +247,7 @@ def is_matroska(path):
         return False
 
 
-class MatroskaFile(object):
+class MatroskaFile(Container):
     """The container structure of a Matroska / WebM file.  `fileobj` (opened unbuffered by default) is any object
     with seek / read; the walk only ever reads through it."""
 
@@ -270,12 +270,6 @@ class MatroskaFile(object):
         if self._own and self._src is not None:
             self._src.f.close()
         self._src = None
-
-    def __enter__(self):
-        return self
-
-    def __exit__(self, *exc):
-        self.close()
 
     @property
     def bytes_read(self):
@@ -668,13 +662,6 @@ class MatroskaFile(object):
             if t.id == sid:
                 return t
         raise SushiError("Stream with index {0} doesn't exist in {1}".format(sid, self.path))
-
-    def streams(self, kind):
-        return [t for t in self.tracks if t.kind == kind]
-
-    def select(self, kind, idx):
-        """The reference's Demuxer._select_stream (demux.py:335-355): kind is 'audio', 'subtitles' or 'video'."""
-        return select_stream(self.streams(kind), kind, idx, self.path)
 
     def select_audio(self, track=None):
         """The audio track `track` (a stream id; None: the reference's default rule).  Its table is released from this

@@ -27,7 +27,7 @@ import struct
 import numpy as np
 
 from . import alac, flac, swr
-from .common import SushiError, select_stream
+from .common import Container, SushiError
 from .matroska import FrameTable, track_audio, track_pcm
 
 MP4_EXTENSIONS = ('.mp4', '.m4a', '.m4v', '.mov')
@@ -128,7 +128,7 @@ class Track(object):
         return '.' + self.codec
 
 
-class Mp4File(object):
+class Mp4File(Container):
     """The box structure of an MP4 / QuickTime file."""
     no_timecodes = 'an MP4 file'                # what the command line says video timestamps cannot be read from
 
@@ -147,12 +147,6 @@ class Mp4File(object):
         if self._f is not None:
             self._f.close()
         self._f = None
-
-    def __enter__(self):
-        return self
-
-    def __exit__(self, *exc):
-        self.close()
 
     def _read(self, pos, n):
         b = os.pread(self._f.fileno(), max(0, min(n, self.size - pos)), pos)
@@ -479,13 +473,6 @@ class Mp4File(object):
                 return t
         raise SushiError("Stream with index {0} doesn't exist in {1}".format(sid, self.path))
 
-    def streams(self, kind):
-        return [t for t in self.tracks if t.kind == kind]
-
-    def select(self, kind, idx):
-        """The reference's Demuxer._select_stream (demux.py:335-355), as MatroskaFile.select."""
-        return select_stream(self.streams(kind), kind, idx, self.path)
-
     def select_audio(self, track=None):
         """The audio track `track` (a stream id; None: the reference's default rule)."""
         t = self.select('audio', track)
@@ -501,9 +488,6 @@ class Mp4File(object):
             label, decode = 'ALAC', alac.track_decoder(t.config)
             fields = swr.audio_format(alac.bit_depth(t.config), swr.ALAC)
         return track_audio(self.path, t.id, label, lambda: self.frames(t), decode, **fields)
-
-    def prefetch(self, payload_ids=(), time_ids=()):
-        """Nothing to read ahead: the audio is read by WavStream, and there is no script or timestamp to read."""
 
     def script_text(self, track):
         raise SushiError('Unknown script type')

@@ -12,20 +12,16 @@ A video stream with neither a PSM entry nor a sequence header at its start is li
 probes its content.  Streams that first appear past the head are not listed.  The audio itself is demuxed and
 decoded on the GPU (sb_ps_*): the host reads the file in large chunks and hands them over, and does no per-packet work.
 """
-import ctypes
 import logging
 import os
 import struct
 
-import numpy as np
-
 from . import _native, swr
-from ._nvtx import nvtx_range
-from .common import Audio, SushiError, select_stream
+from .common import Audio, Container, SushiError
 
 PS_EXTENSIONS = ('.mpg', '.mpeg', '.m2p', '.vob')
 PROBE_SIZE = 5000000             # FFmpeg's default probesize
-# bytes of file each sb_ps_feed call takes; two page-locked buffers of this size
+# bytes of file each sb_ps_feed call takes, through one page-locked buffer
 CHUNK_BYTES = 64 << 20
 
 PSM_TYPES = {0x01: ('video', None), 0x02: ('video', None), 0x03: ('audio', 'mp2'), 0x04: ('audio', 'mp2'),
@@ -113,7 +109,7 @@ class Stream(object):
         return None if h is None else (h >> 17) & 3
 
 
-class ProgramStream(object):
+class ProgramStream(Container):
     """The head of a program stream and its stream list.  `chapters` is always empty (FFmpeg's mpeg demuxer gives
     none)."""
     no_timecodes = 'a program stream'           # what the command line says video timestamps cannot be read from
@@ -126,20 +122,8 @@ class ProgramStream(object):
         if head[:4] != b'\x00\x00\x01\xba' or len(head) < 12 or not (head[4] & 0xC0 == 0x40 or head[4] & 0xF0 == 0x20):
             raise SushiError('{0}: not a program stream (no pack header at its start)'.format(path))
         self.chapters = []
-        self.streams_all = []
+        self.tracks = []
         self._read_head(head)
-
-    def close(self):
-        pass
-
-    def __enter__(self):
-        return self
-
-    def __exit__(self, *exc):
-        self.close()
-
-    def prefetch(self, payload_ids=(), time_ids=()):
-        """Nothing to read ahead: the audio is read by WavStream, and there is no script or timestamp to read."""
 
     def _read_head(self, head):
         psm, found, at = {}, {}, 0
@@ -192,11 +176,11 @@ class ProgramStream(object):
                     continue
             s = found.get(key)
             if s is None:
-                s = found[key] = Stream(len(self.streams_all), key, code, kind, codec)
-                self.streams_all.append(s)
+                s = found[key] = Stream(len(self.tracks), key, code, kind, codec)
+                self.tracks.append(s)
             if code != 0xBD and len(s.head) < 65536:
                 s.head += payload
-        for s in self.streams_all:
+        for s in self.tracks:
             if s.kind == 'video' and s.codec is None:
                 seq = s.head.find(b'\x00\x00\x01\xb3')
                 if seq < 0:
@@ -205,13 +189,6 @@ class ProgramStream(object):
                     ext = s.head.find(b'\x00\x00\x01\xb5', seq)
                     s.codec = 'mpeg2video' if ext >= 0 and s.head[ext + 4] >> 4 == 1 else 'mpeg1video'
 
-    def streams(self, kind):
-        return [s for s in self.streams_all if s.kind == kind]
-
-    def select(self, kind, idx):
-        """The reference's Demuxer._select_stream (demux.py:335-355), as MatroskaFile.select."""
-        return select_stream(self.streams(kind), kind, idx, self.path)
-
     def select_audio(self, track=None):
         s = self.select('audio', track)
         audio_codec(s)
@@ -219,37 +196,9 @@ class ProgramStream(object):
                      **swr.audio_format(16, swr.PLAIN))
 
     def _decode(self, device, s):
-        """The MP2 stream `s`, demuxed and decoded on the GPU (sb_ps_*).  The file is read in chunks of CHUNK_BYTES into
-        two page-locked buffers, one after the other, so that the GPU scans one chunk while the next is read."""
-        lib = _native.lib(device)
-        t = ctypes.c_void_p()
-        _native.check(lib.sb_ps_open(s.pes_id, -1, ctypes.byref(t)), 'sb_ps_open')
-        cut = ctypes.c_int32()
-        try:
-            size = max(1, CHUNK_BYTES)
-            buffers = [_native.pinned_empty((size,), np.uint8) for _ in range(2)]
-            with nvtx_range('sushi_b200: sb_ps_feed'), open(self.path, 'rb', buffering=0) as f:
-                pos, k = 0, 0
-                while True:
-                    view = memoryview(buffers[k % 2])
-                    got = 0
-                    while got < size:
-                        r = f.readinto(view[got:])
-                        if not r:
-                            break
-                        got += r
-                    if got:
-                        arr = buffers[k % 2][:got]
-                        _native.check(lib.sb_ps_feed(t, arr.ctypes.data_as(ctypes.c_void_p), got, pos), 'sb_ps_feed')
-                    pos += got
-                    k += 1
-                    if got < size:
-                        break
-            del buffers
-            h = _native.decode(device, 'sb_ps_finish', t, ctypes.byref(cut))
-        finally:
-            lib.sb_ps_destroy(t)
-        if cut.value:
+        """The MP2 stream `s`, demuxed and decoded on the GPU (sb_ps_*) from chunks of CHUNK_BYTES."""
+        h, cut, _ = _native.demux_file(device, 'sb_ps', (s.pes_id, -1), self.path, CHUNK_BYTES)
+        if cut:
             logging.warning('{0}: stream {1} is cut short at the end of the file; its whole frames are kept, and a last '
                             'frame cut short is decoded with zeros'.format(self.path, s.id))
         return h

@@ -17,20 +17,16 @@ What is kept of FFmpeg's stream rules:
 Only the first PMT version is read: streams a later PMT announces are not listed.  Elementary-stream descriptors
 (languages, stream-level registrations) are not read.  A PAT listing more than one program is refused.
 """
-import ctypes
 import logging
 import os
 
-import numpy as np
-
 from . import _native, swr
-from ._nvtx import nvtx_range
-from .common import Audio, SushiError, select_stream
+from .common import Audio, Container, SushiError
 
 TS_EXTENSIONS = ('.m2ts', '.mts', '.m2t', '.ts')
 PROBE_SIZE = 5000000             # FFmpeg's default probesize: the PAT and the PMT must lie in this many bytes
 SYNC = 0x47
-# bytes of file each sb_ts_feed call takes (rounded down to whole packets); two page-locked buffers of this size
+# bytes of file each sb_ts_feed call takes (rounded down to whole packets), through one page-locked buffer
 CHUNK_BYTES = 64 << 20
 
 ISO_TYPES = {0x01: ('video', 'mpeg2video'), 0x02: ('video', 'mpeg2video'), 0x03: ('audio', 'mp3'),
@@ -82,7 +78,7 @@ class Stream(object):
         return self.codec
 
 
-class TransportStream(object):
+class TransportStream(Container):
     """The head of a transport stream: packet size, program and stream list.  `chapters` is always empty (FFmpeg's
     mpegts demuxer gives none)."""
     no_timecodes = 'a transport stream'         # what the command line says video timestamps cannot be read from
@@ -92,22 +88,9 @@ class TransportStream(object):
         self.size = os.path.getsize(path)
         with open(path, 'rb') as f:
             head = f.read(PROBE_SIZE)
-        self.bytes_read = len(head)
         self.packet_size = self._packet_size(head)
         self.chapters = []
         self._read_tables(head)
-
-    def close(self):
-        pass
-
-    def __enter__(self):
-        return self
-
-    def __exit__(self, *exc):
-        self.close()
-
-    def prefetch(self, payload_ids=(), time_ids=()):
-        """Nothing to read ahead: the audio is read by WavStream, and there is no script or timestamp to read."""
 
     def _packet_size(self, head):
         for size in (192, 188):
@@ -186,7 +169,7 @@ class TransportStream(object):
                 hdmv = True
             at += 2 + n
         self.hdmv = hdmv
-        self.streams_all = []
+        self.tracks = []
         at = 12 + info_len
         while at + 5 <= len(pmt) - 4:
             stype, pid = pmt[at], ((pmt[at + 1] & 0x1F) << 8) | pmt[at + 2]
@@ -194,44 +177,9 @@ class TransportStream(object):
             at += 5 + es_len
             kind, codec = ISO_TYPES.get(stype) or (hdmv and HDMV_TYPES.get(stype)) or MISC_TYPES.get(stype) or \
                 ('other', 'none')
-            self.streams_all.append(Stream(len(self.streams_all), pid, stype, kind, codec))
+            self.tracks.append(Stream(len(self.tracks), pid, stype, kind, codec))
             if hdmv and stype == 0x83:
-                self.streams_all.append(Stream(len(self.streams_all), pid, stype, 'audio', 'ac3'))
-
-    def streams(self, kind):
-        return [s for s in self.streams_all if s.kind == kind]
-
-    def select(self, kind, idx):
-        """The reference's Demuxer._select_stream (demux.py:335-355), as MatroskaFile.select."""
-        return select_stream(self.streams(kind), kind, idx, self.path)
-
-    def chunks(self, buffers):
-        """Read the file into the page-locked `buffers` in turn, whole packets each, yielding (buffer view, byte offset);
-        a buffer is read again only after the next one was handed over.  A partial packet at the end is dropped with a
-        warning."""
-        p = self.packet_size
-        n = max(p, (len(buffers[0]) // p) * p)
-        pos, k = 0, 0
-        with open(self.path, 'rb', buffering=0) as f:
-            while True:
-                view = memoryview(buffers[k % 2])[:n]
-                got = 0
-                while got < n:
-                    r = f.readinto(view[got:])
-                    if not r:
-                        break
-                    got += r
-                whole = got - got % p
-                self.bytes_read += got
-                if got % p:
-                    logging.warning('{0}: the file ends inside the transport stream packet at byte offset {1}; that '
-                                    'packet is dropped'.format(self.path, pos + whole))
-                if whole:
-                    yield view[:whole], pos
-                pos += whole
-                k += 1
-                if got < n:
-                    return
+                self.tracks.append(Stream(len(self.tracks), pid, stype, 'audio', 'ac3'))
 
     def select_audio(self, track=None):
         s = self.select('audio', track)
@@ -241,25 +189,13 @@ class TransportStream(object):
         return Audio(label, s.id, self.path, decode=lambda device: self._decode(device, s), **fields)
 
     def _decode(self, device, s):
-        """The BD-LPCM, TrueHD or MP2 stream `s`, demuxed and decoded on the GPU (sb_ts_*).  The file is read in chunks of
-        CHUNK_BYTES into two page-locked buffers, one after the other, so that the GPU scans one chunk while the next
-        is read."""
-        lib = _native.lib(device)
-        t = ctypes.c_void_p()
-        _native.check(lib.sb_ts_open(self.packet_size, s.pid, DECODED[s.codec][1], ctypes.byref(t)), 'sb_ts_open')
-        cut = ctypes.c_int32()
-        try:
-            size = max(self.packet_size, CHUNK_BYTES // self.packet_size * self.packet_size)
-            buffers = [_native.pinned_empty((size,), np.uint8) for _ in range(2)]
-            with nvtx_range('sushi_b200: sb_ts_feed'):
-                for view, pos in self.chunks(buffers):
-                    arr = np.frombuffer(view, np.uint8)
-                    _native.check(lib.sb_ts_feed(t, arr.ctypes.data_as(ctypes.c_void_p), len(arr), pos), 'sb_ts_feed')
-            del buffers
-            h = _native.decode(device, 'sb_ts_finish', t, ctypes.byref(cut))
-        finally:
-            lib.sb_ts_destroy(t)
-        if cut.value:
+        """The BD-LPCM, TrueHD or MP2 stream `s`, demuxed and decoded on the GPU (sb_ts_*) from chunks of CHUNK_BYTES."""
+        h, cut, dropped = _native.demux_file(device, 'sb_ts', (self.packet_size, s.pid, DECODED[s.codec][1]), self.path,
+                                             CHUNK_BYTES, self.packet_size)
+        if dropped:
+            logging.warning('{0}: the file ends inside the transport stream packet at byte offset {1}; that '
+                            'packet is dropped'.format(self.path, self.size - dropped))
+        if cut:
             logging.warning('{0}: the last PES packet of stream {1} is cut short; its whole sample frames are '
                             'kept'.format(self.path, s.id))
         return h
