@@ -39,7 +39,7 @@
 extern "C" {
 #endif
 
-#define SB_ABI_VERSION 14
+#define SB_ABI_VERSION 15
 
 /* status codes */
 #define SB_OK            0
@@ -56,6 +56,7 @@ typedef struct sb_stream sb_stream;      /* opaque: one normalised stream in HBM
 typedef struct sb_pcm sb_pcm;            /* opaque: decoded interleaved int16 PCM on the device */
 typedef struct sb_ts sb_ts;              /* opaque: one audio PID of an MPEG transport stream being demuxed */
 typedef struct sb_ps sb_ps;              /* opaque: one audio stream of an MPEG program stream being demuxed */
+typedef struct sb_ogg sb_ogg;            /* opaque: one FLAC stream of an Ogg file being demuxed */
 
 /* ---- life cycle ------------------------------------------------------- */
 
@@ -392,6 +393,27 @@ int sb_ps_open(int32_t stream_id, int32_t substream_id, sb_ps** out);
 int sb_ps_feed(sb_ps* ps, const void* host_chunk, int64_t nbytes, int64_t file_offset);
 int sb_ps_finish(sb_ps* ps, int32_t* cut, sb_pcm** out);
 int sb_ps_destroy(sb_ps* ps);
+
+/* ---- Ogg FLAC (ABI version 15) -----------------------------------------------------------------------------------
+ *
+ * The FLAC stream with serial number `serial` of an Ogg file (the FLAC-to-Ogg mapping 1.0: a mapping header packet with
+ * STREAMINFO, then `header_packets` metadata packets, then one FLAC frame per packet), demuxed on the GPU and decoded as
+ * sb_flac_decode_frames decodes listed frames.  channels, bits (16 or 24) and rate come from STREAMINFO.  The file is
+ * fed in chunks of any size, in order; the host does no per-page work.  Pages have variable lengths and may straddle
+ * chunks: every capture pattern of a chunk is found, each links to the one its page's length reaches, and the chain
+ * from the position the previous chunk reached is found by pointer jumping; capture patterns inside page bodies lie
+ * off the chain.  Every page on the chain has its CRC-32 checked.  The chosen stream's pages are checked for sequence
+ * numbers that follow each other and continuation flags that agree with the packet the page before left open, and
+ * their bodies are appended to the stream whose packets sb_ogg_finish decodes; messages about a frame name the file
+ * offset of the page where its packet starts.  Damage fails with SB_EINVAL naming the byte offset: a position the
+ * chain reaches that holds no capture pattern, a version byte other than 0, a CRC mismatch, a sequence gap, a
+ * continuation flag that contradicts the open packet, a page beginning a stream after the first data page (chained
+ * Ogg).  A file cut inside a page drops that page and the packet it leaves open, and sets *cut.  sb_ogg_feed returns
+ * once the chunk is copied and scanned for capture patterns.  The sb_pcm outlives the sb_ogg. */
+int sb_ogg_open(uint32_t serial, int32_t channels, int32_t bits, int32_t rate, int32_t header_packets, sb_ogg** out);
+int sb_ogg_feed(sb_ogg* ogg, const void* host_chunk, int64_t nbytes, int64_t file_offset);
+int sb_ogg_finish(sb_ogg* ogg, int32_t* cut, sb_pcm** out);
+int sb_ogg_destroy(sb_ogg* ogg);
 
 /* ---- multi-GPU: events shard across ranks (SURVEY.md 8e) ---------------- */
 

@@ -1,5 +1,6 @@
-// What the demultiplexers fed a file in chunks (sb_ts.cu, sb_ps.cu) share, written once: the device scans of per-CTA
-// totals, the device buffers that grow with the stream, and the host-side life of a handle (open, feed checks, waiting
+// What the demultiplexers fed a file in chunks (sb_ts.cu, sb_ps.cu, sb_ogg.cu) share, written once: the device scans
+// of per-CTA totals, the chain of variable-length packets by pointer jumping, the device buffers that grow with the
+// stream, and the host-side life of a handle (open, feed checks, waiting
 // for the last chunk, the refusal of the first failure, destroy).  Host and device code, not part of the ABI; each
 // translation unit keeps its own copy.
 #pragma once
@@ -68,6 +69,44 @@ k_scan_totals(long long* __restrict__ cta, int64_t n_cta, const long long* base,
 #pragma unroll
         for (int k = 0; k < N; ++k) total[k] = run[k];
     }
+}
+
+// ---- the packet chain of a chunk (sb_ps.cu, sb_ogg.cu) ----------------------------------------------------------
+// Candidates are the positions pos[0, m) (sorted) where a packet or page may start; each links to the candidate its
+// length reaches, or to the sink m where the chain ends.  The chain from candidate 0 is marked by pointer jumping.
+
+// the candidate at position p, or -1
+__device__ __forceinline__ int64_t find_cand(const int64_t* __restrict__ pos, int64_t m, int64_t p) {
+    int64_t lo = 0, hi = m;
+    while (lo < hi) {
+        const int64_t mid = (lo + hi) >> 1;
+        if (pos[mid] < p) lo = mid + 1; else hi = mid;
+    }
+    return lo < m && pos[lo] == p ? lo : -1;
+}
+
+// one round: every marked candidate marks the one `span` links on; the links double.  A mark set during the round
+// is on the chain too, so reading it early only marks more of the chain sooner.
+__global__ void __launch_bounds__(kThreads)
+k_chain_jump(const int32_t* __restrict__ jin, int32_t* __restrict__ jout, uint8_t* on, int64_t m) {
+    const int64_t v = (int64_t)blockIdx.x * blockDim.x + threadIdx.x;
+    if (v > m) return;
+    const int32_t j = jin[v];
+    if (on[v]) on[j] = 1;
+    jout[v] = jin[j];
+}
+
+// the rounds of k_chain_jump until 2^r covers the longest chain, m links; jump[0] holds the links (jump[m] == m) and
+// on[] the chain's start, and each round is counted as `prof_name`
+inline cudaError_t mark_chain(int32_t* const jump[2], uint8_t* on, int64_t m, const char* prof_name, cudaStream_t st) {
+    const unsigned j_cta = (unsigned)((m + 1 + kThreads - 1) / kThreads);
+    cudaError_t e = cudaSuccess;
+    for (int r = 0; e == cudaSuccess && ((int64_t)1 << r) < m; ++r) {
+        ProfScope ps(prof_name);
+        k_chain_jump<<<j_cta, kThreads, 0, st>>>(jump[r & 1], jump[(r & 1) ^ 1], on, m);
+        e = cudaGetLastError();
+    }
+    return e;
 }
 
 // exclusive scan of n int64 values in place: tile sums, one CTA over the tiles, then each tile

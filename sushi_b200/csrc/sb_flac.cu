@@ -88,7 +88,7 @@ namespace {
 // A FLAC input on the device and its frame table while it is decoded; the upload is freed with it
 struct FlacInput {
     Blocks blocks;
-    uint8_t* d_file = nullptr;
+    const uint8_t* d_file = nullptr;
     int64_t nbytes = 0;
     int channels = 0, bits = 0, framerate = 0;
     std::vector<FrameDesc> frames;
@@ -138,7 +138,61 @@ int decode(const FlacInput& h, sb_pcm** out, const char* who) {
     return pcm_handle(blocks.take(d_pcm), h.samples, ch, h.framerate, out);
 }
 
+// the stream parameters, and the listed frames: a frame ends where the next one starts, so the frame named is the one
+// that starts at or before its predecessor
+int check_listed(const int64_t* offsets, const int64_t* file_offsets, int64_t n, int64_t nbytes, int channels, int bits,
+                 int framerate, const char* who) {
+    if (bits != 16 && bits != 24) SB_FAIL(SB_EINVAL, "FLAC with %d bits per sample is not supported (16 or 24)", bits);
+    if (channels < 1 || channels > 8 || framerate < 1 || nbytes < 1 || n < 0)
+        SB_FAIL(SB_EINVAL, "%s: bad stream parameters", who);
+    for (int64_t f = 0; f < n; ++f)
+        if (offsets[f] < 0 || offsets[f] >= nbytes || (f > 0 && offsets[f] <= offsets[f - 1]))
+            SB_FAIL(SB_EINVAL, "FLAC frame %lld at byte offset %lld: %s", (long long)f, (long long)file_offsets[f],
+                    offsets[f] < 0 || offsets[f] >= nbytes ? "frame starts outside the buffer" : "empty frame");
+    return SB_OK;
+}
+
+// after check_listed: k_flac_frames on the listed frames, their table, then decode
+int decode_listed(const uint8_t* d_buf, int64_t nbytes, const int64_t* d_offsets, const int64_t* offsets,
+                  const int64_t* file_offsets, int64_t n, int channels, int bits, int framerate, sb_pcm** out,
+                  const char* who) {
+    Ctx& c = ctx();
+    FlacInput h;
+    h.d_file = d_buf;
+    h.nbytes = nbytes; h.channels = channels; h.bits = bits; h.framerate = framerate;
+    h.where = file_offsets;
+    std::vector<sbflac::ListedFrame> listed((size_t)n);
+    {
+        Blocks blocks;
+        sbflac::ListedFrame* d_listed = nullptr;
+        SB_TRY(blocks.alloc(&d_listed, (size_t)n));
+        cudaError_t e = cudaSuccess;
+        if (n > 0) {
+            ProfScope ps("flac_frames");
+            k_flac_frames<<<(unsigned)((n + 255) / 256), 256, 0, c.stream>>>(d_buf, nbytes, d_offsets, n, channels,
+                                                                             bits, framerate, d_listed);
+            e = cudaGetLastError();
+        }
+        SB_TRY(collect(e, listed.data(), d_listed, n, who));
+    }
+    char msg[256];
+    if (!sbflac::list_frames(listed.data(), offsets, file_offsets, n, nbytes, h.frames, &h.samples, msg, sizeof(msg)))
+        SB_FAIL(SB_EINVAL, "%s", msg);
+    return decode(h, out, who);
+}
+
 }  // namespace
+
+namespace sb {
+
+int flac_decode(const uint8_t* d_buf, int64_t nbytes, const int64_t* d_offsets, const int64_t* offsets,
+                const int64_t* file_offsets, int64_t n, int channels, int bits, int framerate, sb_pcm** out,
+                const char* who) {
+    SB_TRY(check_listed(offsets, file_offsets, n, nbytes, channels, bits, framerate, who));
+    return decode_listed(d_buf, nbytes, d_offsets, offsets, file_offsets, n, channels, bits, framerate, out, who);
+}
+
+}  // namespace sb
 
 extern "C" {
 
@@ -153,7 +207,9 @@ int sb_flac_decode_file(const void* file, int64_t nbytes, int64_t first_frame_of
     FlacInput h;
     h.nbytes = nbytes; h.channels = channels; h.bits = bits; h.framerate = framerate;
     const uint8_t* host = static_cast<const uint8_t*>(file);
-    SB_TRY(upload_padded(h.blocks, &h.d_file, file, nbytes, who));
+    uint8_t* d_file = nullptr;
+    SB_TRY(upload_padded(h.blocks, &d_file, file, nbytes, who));
+    h.d_file = d_file;
 
     // candidates: a frame has at least 9 bytes; real files hold one frame per few kB and false syncs are rarer still
     std::vector<Candidate> cand;
@@ -175,38 +231,14 @@ int sb_flac_decode_frames(const void* buf, int64_t nbytes, const int64_t* offset
     const char* who = "sb_flac_decode_frames";
     Ctx& c = ctx();
     SB_TRY(entry_check(who, buf && offsets && file_offsets && out));
-    if (bits != 16 && bits != 24) SB_FAIL(SB_EINVAL, "FLAC with %d bits per sample is not supported (16 or 24)", bits);
-    if (channels < 1 || channels > 8 || framerate < 1 || nbytes < 1 || n < 0)
-        SB_FAIL(SB_EINVAL, "sb_flac_decode_frames: bad stream parameters");
-    // a frame ends where the next one starts: here the frame named is the one that starts at or before its predecessor
-    for (int64_t f = 0; f < n; ++f)
-        if (offsets[f] < 0 || offsets[f] >= nbytes || (f > 0 && offsets[f] <= offsets[f - 1]))
-            SB_FAIL(SB_EINVAL, "FLAC frame %lld at byte offset %lld: %s", (long long)f, (long long)file_offsets[f],
-                    offsets[f] < 0 || offsets[f] >= nbytes ? "frame starts outside the buffer" : "empty frame");
-    FlacInput h;
-    h.nbytes = nbytes; h.channels = channels; h.bits = bits; h.framerate = framerate;
-    h.where = file_offsets;
-    SB_TRY(upload_padded(h.blocks, &h.d_file, buf, nbytes, who));
-    std::vector<sbflac::ListedFrame> listed((size_t)n);
-    {
-        Blocks blocks;
-        int64_t* d_offsets = nullptr;
-        sbflac::ListedFrame* d_listed = nullptr;
-        SB_TRY(blocks.alloc(&d_offsets, (size_t)n));
-        SB_TRY(blocks.alloc(&d_listed, (size_t)n));
-        cudaError_t e = cudaMemcpyAsync(d_offsets, offsets, sizeof(int64_t) * n, cudaMemcpyHostToDevice, c.stream);
-        if (e == cudaSuccess && n > 0) {
-            ProfScope ps("flac_frames");
-            k_flac_frames<<<(unsigned)((n + 255) / 256), 256, 0, c.stream>>>(h.d_file, nbytes, d_offsets, n, channels,
-                                                                             bits, framerate, d_listed);
-            e = cudaGetLastError();
-        }
-        SB_TRY(collect(e, listed.data(), d_listed, n, who));
-    }
-    char msg[256];
-    if (!sbflac::list_frames(listed.data(), offsets, file_offsets, n, nbytes, h.frames, &h.samples, msg, sizeof(msg)))
-        SB_FAIL(SB_EINVAL, "%s", msg);
-    return decode(h, out, who);
+    SB_TRY(check_listed(offsets, file_offsets, n, nbytes, channels, bits, framerate, who));
+    Blocks blocks;
+    uint8_t* d_buf = nullptr;
+    int64_t* d_offsets = nullptr;
+    SB_TRY(upload_padded(blocks, &d_buf, buf, nbytes, who));
+    SB_TRY(blocks.alloc(&d_offsets, (size_t)n));
+    SB_TRY(cuda_result(cudaMemcpyAsync(d_offsets, offsets, sizeof(int64_t) * n, cudaMemcpyHostToDevice, c.stream), who));
+    return decode_listed(d_buf, nbytes, d_offsets, offsets, file_offsets, n, channels, bits, framerate, out, who);
 }
 
 }  // extern "C"

@@ -149,6 +149,12 @@ int pcm_handle(int16_t* d_pcm, int64_t frames, int channels, int rate, sb_pcm** 
 // offset of stream byte b; *cut 1 when a cut last frame was dropped
 int mp2_decode(const uint8_t* host, const uint8_t* d_buf, int64_t nbytes, const std::function<int64_t(int64_t)>& where,
                int32_t* cut, sb_pcm** out);
+// FLAC (sb_flac.cu): the frames of a stream on the device at d_buf (zero tail of sb_decode.h), frame f starting at
+// offsets[f] (d_offsets its copy on the device) and ending where the next one starts (the last at nbytes);
+// file_offsets[f] is the file offset messages name for it.  sb_flac_decode_frames is an upload and this call.
+int flac_decode(const uint8_t* d_buf, int64_t nbytes, const int64_t* d_offsets, const int64_t* offsets,
+                const int64_t* file_offsets, int64_t n, int channels, int bits, int framerate, sb_pcm** out,
+                const char* who);
 int truehd_index_device(const uint8_t* host, const uint8_t* d_buf, int64_t nbytes, const int64_t* offsets,
                         const int64_t* d_blocks, int64_t n, const std::function<int64_t(int64_t)>& where, sb_pcm** out);
 

@@ -9,8 +9,9 @@
 //                  (the candidate count comes back to size the launches), then
 //                    k_ps_link      one thread per candidate: its packet's length and the candidate it links to (or how
 //                                   the chain ends there)
-//                    k_ps_jump      log2(candidates) rounds of pointer jumping from the chunk's first position: each
+//                    k_chain_jump   log2(candidates) rounds of pointer jumping from the chunk's first position: each
 //                                   round, every candidate on the chain marks the one 2^r links on, and the links double
+//                                   (sb_demux.cuh)
 //                    k_ps_pes       one thread per candidate on the chain: the chain's end (the next chunk's carry, or a
 //                                   refusal), the chosen stream's PES header, per-CTA payload totals
 //                    k_scan_totals  one CTA: their exclusive scan on top of the running totals
@@ -65,16 +66,6 @@ k_ps_cands(const uint8_t* __restrict__ buf, int64_t limit, const long long* __re
     for (; m; m &= m - 1) pos[at++] = i0 + __ffs(m) - 1;
 }
 
-// the candidate at position p, or -1
-__device__ __forceinline__ int64_t find_cand(const int64_t* __restrict__ pos, int64_t m, int64_t p) {
-    int64_t lo = 0, hi = m;
-    while (lo < hi) {
-        const int64_t mid = (lo + hi) >> 1;
-        if (pos[mid] < p) lo = mid + 1; else hi = mid;
-    }
-    return lo < m && pos[lo] == p ? lo : -1;
-}
-
 // node m is the sink every chain end links to; jump[] starts as the links
 __global__ void __launch_bounds__(kThreads)
 k_ps_link(const uint8_t* __restrict__ buf, int64_t n, int64_t limit, int at_end, int64_t file_off0,
@@ -93,17 +84,6 @@ k_ps_link(const uint8_t* __restrict__ buf, int64_t n, int64_t limit, int at_end,
     links[k] = l;
     jump[k] = (int32_t)(l.kind == sbps::kLink ? find_cand(pos, m, l.next) : m);
     on[k] = k == 0 && pos[0] == 0;
-}
-
-// one round: every marked candidate marks the one `span` links on; the links double.  A mark set during the round
-// is on the chain too, so reading it early only marks more of the chain sooner.
-__global__ void __launch_bounds__(kThreads)
-k_ps_jump(const int32_t* __restrict__ jin, int32_t* __restrict__ jout, uint8_t* on, int64_t m) {
-    const int64_t v = (int64_t)blockIdx.x * blockDim.x + threadIdx.x;
-    if (v > m) return;
-    const int32_t j = jin[v];
-    if (on[v]) on[j] = 1;
-    jout[v] = jin[j];
 }
 
 // one thread per candidate: on the chain, the chosen stream's PES payload; the chain's end
@@ -238,14 +218,7 @@ int scan_buffer(sb_ps* t, const uint8_t* buf, int64_t n, int64_t base, bool at_e
                                                              t->d_jump[0], t->d_on, t->d_run, t->d_err);
         e = cudaGetLastError();
     }
-    // rounds until 2^r covers the longest chain, m links
-    const unsigned j_cta = (unsigned)((m + 1 + kThreads - 1) / kThreads);
-    int r = 0;
-    for (; e == cudaSuccess && ((int64_t)1 << r) < m; ++r) {
-        ProfScope ps("ps_chain");
-        k_ps_jump<<<j_cta, kThreads, 0, c.stream>>>(t->d_jump[r & 1], t->d_jump[(r & 1) ^ 1], t->d_on, m);
-        e = cudaGetLastError();
-    }
+    if (e == cudaSuccess) e = mark_chain(t->d_jump, t->d_on, m, "ps_chain", c.stream);
     if (e == cudaSuccess) {
         ProfScope ps("ps_compact", 4);
         k_ps_pes<<<(unsigned)m_cta, kThreads, 0, c.stream>>>(buf, n, at_end, base, t->stream_id, t->d_pos, m, t->d_links,

@@ -3,7 +3,7 @@ them all) with one method, select_audio(track=None), which makes every refusal t
 common.Audio WavStream loads.  WavStream detects the format (open_input); the command line goes by file extension."""
 import collections
 
-from . import matroska, mp4, mpa, mpegps, mpegts, truehd, tta, wavpack
+from . import matroska, mp4, mpa, mpegps, mpegts, ogg, truehd, tta, wavpack
 from .flac import FlacFile, is_flac
 from .wav import DownmixedWavFile
 
@@ -23,18 +23,24 @@ FORMATS = (
     Format('WAV', ('.wav',), lambda path: True, DownmixedWavFile, None),      # whatever is nothing else
 )
 # The MPEG systems whose audio is MP2: program streams and raw MPEG audio, both known by their names.  They are asked
-# before the table above; READERS is the whole table, in the order open_input asks.
+# before the table above.
 MPEG_FORMATS = (
     Format('program stream', mpegps.PS_EXTENSIONS, mpegps.is_program_stream, mpegps.ProgramStream,
            'a program stream'),
     Format('MPEG audio', mpa.MPA_EXTENSIONS, mpa.is_mpeg_audio, mpa.MpegAudioFile, None),
 )
-READERS = MPEG_FORMATS + FORMATS
+# Ogg files, known by their capture pattern, asked after those and before the table above
+OGG_FORMATS = (
+    Format('Ogg', ogg.OGG_EXTENSIONS, ogg.is_ogg, ogg.OggFile, 'an Ogg file'),
+)
+# READERS is the whole table, in the order open_input asks.
+READERS = MPEG_FORMATS + OGG_FORMATS + FORMATS
 
 
 def open_input(source):
     """(reader, format name) of `source`: a file name, whose format is detected by content, or an opened container
-    reader (MatroskaFile, Mp4File, TransportStream, ProgramStream), which is returned as it is and never sniffed."""
+    reader (MatroskaFile, Mp4File, TransportStream, ProgramStream, OggFile), which is returned as it is and never
+    sniffed."""
     for f in READERS:
         if f.opens_as and isinstance(source, f.reader):
             return source, f.name
