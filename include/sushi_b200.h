@@ -39,7 +39,7 @@
 extern "C" {
 #endif
 
-#define SB_ABI_VERSION 15
+#define SB_ABI_VERSION 16
 
 /* status codes */
 #define SB_OK            0
@@ -323,6 +323,21 @@ int sb_wavpack_decode_blocks(const void* buf, int64_t nbytes, const int64_t* tab
  * that reaches the last frame's length with only its CRC left (FFmpeg's decoder cuts such a frame short); bytes left
  * between the last sample and the CRC; a CRC that disagrees. */
 int sb_tta_decode_frames(const void* buf, int64_t nbytes, const int64_t* offsets, const int64_t* file_offsets, int64_t n,
+                         const int32_t* config, sb_pcm** out);
+
+/* Monkey's Audio, APE (ABI version 16): FFmpeg's `ape` decoder output for file version 3990 (Monkey's Audio 3.99 and
+ * later), compression levels 1000 to 5000, 16 or 24 bits, mono or stereo; 24-bit samples by the top 16 bits of
+ * FFmpeg's S32 sample.  `buf` holds the file's bytes up to `nbytes` (the file less its stored WAV tail): frame f starts
+ * at offsets[f] (its seek-table position plus any ID3v2 tag in front; increasing), and, as FFmpeg's demuxer cuts it,
+ * runs to the next frame's start, the last to nbytes; the frames are 32-bit little-endian words counted from frame 0.
+ * file_offsets[f] is what an error names with the frame index.  config[0..5] is channels (1 or 2), bits (16 or 24),
+ * rate, compression level, blocks per frame and the last frame's blocks.  The decode runs in stages over an int32
+ * scratch of every sample: the range decoder (one thread per frame), the NN filters (one warp per frame and channel),
+ * the predictor (one thread per frame) and the frame CRC (one warp per frame).  It fails on: a frame header cut short;
+ * frame flags other than mono silence, stereo silence and pseudo-stereo; a range decoder that reads past its frame or
+ * meets a symbol past 65535; a CRC that disagrees (FFmpeg checks it only under AV_EF_CRCCHECK); a 24-bit stereo sample
+ * past 24 bits (where FFmpeg switches to its 64-bit predictor). */
+int sb_ape_decode_frames(const void* buf, int64_t nbytes, const int64_t* offsets, const int64_t* file_offsets, int64_t n,
                          const int32_t* config, sb_pcm** out);
 
 /* MPEG-1/2 audio layer II, MP2 (ABI version 13): FFmpeg's fixed-point `mp2` decoder output, bit for bit, 1 or 2

@@ -3,7 +3,7 @@ them all) with one method, select_audio(track=None), which makes every refusal t
 common.Audio WavStream loads.  WavStream detects the format (open_input); the command line goes by file extension."""
 import collections
 
-from . import matroska, mp4, mpa, mpegps, mpegts, ogg, truehd, tta, wavpack
+from . import ape, matroska, mp4, mpa, mpegps, mpegts, ogg, truehd, tta, wavpack
 from .flac import FlacFile, is_flac
 from .wav import DownmixedWavFile
 
@@ -33,8 +33,13 @@ MPEG_FORMATS = (
 OGG_FORMATS = (
     Format('Ogg', ogg.OGG_EXTENSIONS, ogg.is_ogg, ogg.OggFile, 'an Ogg file'),
 )
+# Monkey's Audio files, known by their `MAC ` marker (after an optional ID3v2 tag), asked after those and before the
+# table above
+APE_FORMATS = (
+    Format('APE', ape.APE_EXTENSIONS, ape.is_ape, ape.ApeFile, None),
+)
 # READERS is the whole table, in the order open_input asks.
-READERS = MPEG_FORMATS + OGG_FORMATS + FORMATS
+READERS = MPEG_FORMATS + OGG_FORMATS + APE_FORMATS + FORMATS
 
 
 def open_input(source):

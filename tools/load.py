@@ -29,8 +29,8 @@ import numpy as np  # noqa: E402
 
 from sushi_b200 import _native, matroska, mp4, mpegts, tta, wavpack  # noqa: E402
 from sushi_b200.wavstream import FlacFile, WavStream  # noqa: E402
-from tests import (alac_cases, flac_cases as fc, loader_cases as lc, mkv_cases, mp2_cases, mp4_cases, ogg_cases,  # noqa
-                   ps_cases, ref_mp2, ref_swr, truehd_cases, ts_cases, tta_cases, wavpack_cases)
+from tests import (alac_cases, ape_cases, flac_cases as fc, loader_cases as lc, mkv_cases, mp2_cases,  # noqa
+                   mp4_cases, ogg_cases, ps_cases, ref_mp2, ref_swr, truehd_cases, ts_cases, tta_cases, wavpack_cases)
 
 
 # ---- what every format shares ------------------------------------------------------------------------------------
@@ -336,6 +336,19 @@ def build_tta(directory, minutes, bits):
     return sized({'minutes': minutes, 'bits': bits}, ('tta', path), ('flac', flac), ('wav', wav))
 
 
+def build_ape(directory, minutes, bits):
+    """tests/ape_cases.py's long stream (one insane-level frame of the size Monkey's Audio writes, 1 179 648 blocks,
+    repeated), the WAV of the same samples, and write_flac's file (other audio of the same shape)."""
+    case, data, reps = ape_cases.long_stream(bits=bits, minutes=minutes)
+    path = write(os.path.join(directory, 'ape%d_%d.ape' % (minutes, bits)), data)
+    del data
+    wav = write_wav(os.path.join(directory, 'ape%d_%d.wav' % (minutes, bits)), case.pcm, reps, case.pcm[:0],
+                    bits // 8)
+    flac = write_flac(directory, minutes, bits)[0]
+    return sized({'minutes': minutes, 'bits': bits, 'frame_blocks': case.bpf, 'frames': reps}, ('ape', path),
+                 ('flac', flac), ('wav', wav))
+
+
 PS_PACK = 2048
 PS_VIDEO_PER_AUDIO = 11              # video packs between audio packs: about 1.5 GB for 90 minutes
 
@@ -511,9 +524,14 @@ FORMATS = {
 }
 
 
+# Every format the tool measures: FORMATS, and the formats added after tests/test_load_tool.py's table of input kinds,
+# which tests/test_load_tool_ape.py builds in the same way.
+ALL_FORMATS = dict(FORMATS, ape=Format((24, 90), (16, 24), build_ape))
+
+
 def cases(name, minutes, bits):
     """[(minutes, bits)] of one format: its defaults, or those asked for when it can build them."""
-    fmt = FORMATS[name]
+    fmt = ALL_FORMATS[name]
     out = [(m, b) for m in minutes or fmt.minutes for b in ([None] if fmt.bits is None else bits or fmt.bits)]
     for m, b in out:
         if m < 1:
@@ -545,7 +563,7 @@ def measure(lib, files, runs):
 
 def main():
     ap = argparse.ArgumentParser(description=__doc__.splitlines()[0])
-    ap.add_argument('formats', nargs='+', choices=list(FORMATS), metavar='FORMAT', help=' '.join(FORMATS))
+    ap.add_argument('formats', nargs='+', choices=list(ALL_FORMATS), metavar='FORMAT', help=' '.join(ALL_FORMATS))
     ap.add_argument('--minutes', type=int, nargs='+')
     ap.add_argument('--bits', type=int, nargs='+')
     ap.add_argument('--runs', type=int, default=3)
@@ -563,10 +581,10 @@ def main():
         for name, todo in plan:
             print(json.dumps({'format': name, 'card': card(), 'sms': sms}), flush=True)
             for minutes, bits in todo:
-                files = FORMATS[name].build(directory, minutes, bits)
+                files = ALL_FORMATS[name].build(directory, minutes, bits)
                 measure(lib, files, args.runs)
-                if FORMATS[name].extra:
-                    FORMATS[name].extra(lib, minutes, args.runs)
+                if ALL_FORMATS[name].extra:
+                    ALL_FORMATS[name].extra(lib, minutes, args.runs)
                 for path in {path for _, path in files}:
                     os.remove(path)
             print(json.dumps({'card_after': card()}), flush=True)
