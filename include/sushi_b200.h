@@ -39,7 +39,7 @@
 extern "C" {
 #endif
 
-#define SB_ABI_VERSION 16
+#define SB_ABI_VERSION 17
 
 /* status codes */
 #define SB_OK            0
@@ -339,6 +339,23 @@ int sb_tta_decode_frames(const void* buf, int64_t nbytes, const int64_t* offsets
  * past 24 bits (where FFmpeg switches to its 64-bit predictor). */
 int sb_ape_decode_frames(const void* buf, int64_t nbytes, const int64_t* offsets, const int64_t* file_offsets, int64_t n,
                          const int32_t* config, sb_pcm** out);
+
+/* TAK (ABI version 17): FFmpeg's `tak` decoder output for integer TAK of 16 or 24 bits, 1 to 6 channels, codec types
+ * mono/stereo and multichannel; 24-bit samples by the top 16 bits of FFmpeg's S32 sample.  `file` holds the whole
+ * file (nbytes bytes); its frames lie in [audio_start, audio_end) (audio_end: LAST_FRAME's end, a trailing APEv2 or
+ * ID3v1 tag, or the end of the file).  config[0..7] is channels, bits, rate, codec type, frame size type, the total
+ * samples per channel (low and high 32 bits) and the channel mask, all from STREAMINFO.  Frames start where FFmpeg's
+ * tak parser starts them (sync word, a header that parses, its CRC-24), found on the GPU; they must be numbered from
+ * 0, start at audio_start and follow each other with no byte between, the first carry stream info, every stream info
+ * agree with config, and the lengths add up to the total.  The decode runs in stages over an int32 scratch of every
+ * sample: the residual codes (one thread per frame), the prediction filters (one warp per frame and channel), the
+ * decorrelation, lpc scans and store (one CTA per frame) and the data CRC (one warp per frame).  It fails, naming the
+ * frame and its byte offset, on: a read past the frame; a subframe layout, filter order or residual coding FFmpeg
+ * rejects; a sample shift at or above the bit depth; filtered decorrelation on fewer than 256 samples; multichannel
+ * decorrelation parameters FFmpeg rejects or that leave a channel undecoded; the frame metadata flag; bytes after the
+ * data CRC; a data CRC that disagrees (FFmpeg checks it only under AV_EF_CRCCHECK). */
+int sb_tak_decode_file(const void* file, int64_t nbytes, int64_t audio_start, int64_t audio_end, const int32_t* config,
+                       sb_pcm** out);
 
 /* MPEG-1/2 audio layer II, MP2 (ABI version 13): FFmpeg's fixed-point `mp2` decoder output, bit for bit, 1 or 2
  * channels at 16 to 48 kHz.  `buf` holds a Matroska track's block payloads back to back (block k at offsets[k], at

@@ -17,7 +17,7 @@ LIB_PATH = os.path.join(_HERE, 'libsushi_b200.so')
 
 SB_OK = 0
 SB_U8, SB_F32 = 0, 1
-ABI_VERSION = 16
+ABI_VERSION = 17
 SB_TS_PCM_BLURAY, SB_TS_TRUEHD, SB_TS_MP2 = 0, 1, 2
 
 c_i64 = ctypes.c_int64
@@ -85,6 +85,7 @@ PROTOTYPES = {
                                                 ctypes.POINTER(c_vp)]),
     'sb_tta_decode_frames': (ctypes.c_int, [c_vp, c_i64, c_i64p, c_i64p, c_i64, c_i32p, ctypes.POINTER(c_vp)]),
     'sb_ape_decode_frames': (ctypes.c_int, [c_vp, c_i64, c_i64p, c_i64p, c_i64, c_i32p, ctypes.POINTER(c_vp)]),
+    'sb_tak_decode_file': (ctypes.c_int, [c_vp, c_i64, c_i64, c_i64, c_i32p, ctypes.POINTER(c_vp)]),
     'sb_mp2_decode_frames': (ctypes.c_int, [c_vp, c_i64, c_i64p, c_i64p, c_i64, ctypes.POINTER(c_vp)]),
     'sb_mp2_decode_stream': (ctypes.c_int, [c_vp, c_i64, c_i64, c_i32p, ctypes.POINTER(c_vp)]),
     'sb_ts_open': (ctypes.c_int, [ctypes.c_int, ctypes.c_int32, ctypes.c_int32, ctypes.POINTER(c_vp)]),

@@ -109,9 +109,9 @@ def create_arg_parser():
                         help='Timecodes file to use instead of making one from the source (when possible)')
 
     parser.add_argument('--src', required=True, dest='source', metavar='<filename>',
-                        help='Source audio or video (WAV, FLAC, WavPack, TTA, APE, TrueHD, Matroska, MP4, MPEG-TS or Ogg)')
+                        help='Source audio or video (WAV, FLAC, WavPack, TTA, APE, TAK, TrueHD, Matroska, MP4, MPEG-TS or Ogg)')
     parser.add_argument('--dst', required=True, dest='destination', metavar='<filename>',
-                        help='Destination audio or video (WAV, FLAC, WavPack, TTA, APE, TrueHD, Matroska, MP4, MPEG-TS or Ogg)')
+                        help='Destination audio or video (WAV, FLAC, WavPack, TTA, APE, TAK, TrueHD, Matroska, MP4, MPEG-TS or Ogg)')
     parser.add_argument('-o', '--output', default=None, dest='output_script', metavar='<filename>',
                         help='Output script')
 
@@ -124,7 +124,7 @@ def create_arg_parser():
 def _open_input(path):
     """The opened reader of a container input (inputs.READERS: Matroska, MP4, Ogg, transport or program stream), which also
     gives its script, chapters and streams; None for a WAV, FLAC, raw TrueHD (.thd), WavPack (.wv), TTA (.tta), Monkey's
-    Audio (.ape) or MPEG audio (.mp2, .mpa, .m2a) input,
+    Audio (.ape), TAK (.tak) or MPEG audio (.mp2, .mpa, .m2a) input,
     which WavStream reads.  Any other extension, or a container's that does not open as one, is refused where the
     reference would have ffmpeg demux it."""
     ext = get_extension(path)
@@ -133,7 +133,7 @@ def _open_input(path):
     if fmt is None:
         raise SushiError(refusal)
     if fmt.opens_as is None:
-        if fmt.name in ('WavPack', 'TTA', 'APE', 'MPEG audio'):
+        if fmt.name in ('WavPack', 'TTA', 'APE', 'TAK', 'MPEG audio'):
             fmt.reader(path)                       # its refusals, before the GPU is touched
         return None
     try:

@@ -3,7 +3,7 @@ them all) with one method, select_audio(track=None), which makes every refusal t
 common.Audio WavStream loads.  WavStream detects the format (open_input); the command line goes by file extension."""
 import collections
 
-from . import ape, matroska, mp4, mpa, mpegps, mpegts, ogg, truehd, tta, wavpack
+from . import ape, matroska, mp4, mpa, mpegps, mpegts, ogg, tak, truehd, tta, wavpack
 from .flac import FlacFile, is_flac
 from .wav import DownmixedWavFile
 
@@ -38,8 +38,12 @@ OGG_FORMATS = (
 APE_FORMATS = (
     Format('APE', ape.APE_EXTENSIONS, ape.is_ape, ape.ApeFile, None),
 )
+# TAK files, known by their `tBaK` marker (after an optional ID3v2 tag), asked after those and before the table above
+TAK_FORMATS = (
+    Format('TAK', tak.TAK_EXTENSIONS, tak.is_tak, tak.TakFile, None),
+)
 # READERS is the whole table, in the order open_input asks.
-READERS = MPEG_FORMATS + OGG_FORMATS + APE_FORMATS + FORMATS
+READERS = MPEG_FORMATS + OGG_FORMATS + APE_FORMATS + TAK_FORMATS + FORMATS
 
 
 def open_input(source):

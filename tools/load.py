@@ -30,7 +30,8 @@ import numpy as np  # noqa: E402
 from sushi_b200 import _native, matroska, mp4, mpegts, tta, wavpack  # noqa: E402
 from sushi_b200.wavstream import FlacFile, WavStream  # noqa: E402
 from tests import (alac_cases, ape_cases, flac_cases as fc, loader_cases as lc, mkv_cases, mp2_cases,  # noqa
-                   mp4_cases, ogg_cases, ps_cases, ref_mp2, ref_swr, truehd_cases, ts_cases, tta_cases, wavpack_cases)
+                   mp4_cases, ogg_cases, ps_cases, ref_mp2, ref_swr, tak_cases, truehd_cases, ts_cases, tta_cases,
+                   wavpack_cases)
 
 
 # ---- what every format shares ------------------------------------------------------------------------------------
@@ -349,6 +350,19 @@ def build_ape(directory, minutes, bits):
                  ('flac', flac), ('wav', wav))
 
 
+def build_tak(directory, minutes, bits):
+    """tests/tak_cases.py's long stream (one 250 ms frame at the largest filter order, repeated with its own frame
+    numbers), the WAV of the same samples, and write_flac's file (other audio of the same shape)."""
+    case, data, reps = tak_cases.long_stream(bits=bits, minutes=minutes)
+    path = write(os.path.join(directory, 'tak%d_%d.tak' % (minutes, bits)), data)
+    del data
+    wav = write_wav(os.path.join(directory, 'tak%d_%d.wav' % (minutes, bits)), case.pcm, reps, case.pcm[:0],
+                    bits // 8)
+    flac = write_flac(directory, minutes, bits)[0]
+    return sized({'minutes': minutes, 'bits': bits, 'frame_samples': case.nb, 'frames': reps}, ('tak', path),
+                 ('flac', flac), ('wav', wav))
+
+
 PS_PACK = 2048
 PS_VIDEO_PER_AUDIO = 11              # video packs between audio packs: about 1.5 GB for 90 minutes
 
@@ -525,8 +539,8 @@ FORMATS = {
 
 
 # Every format the tool measures: FORMATS, and the formats added after tests/test_load_tool.py's table of input kinds,
-# which tests/test_load_tool_ape.py builds in the same way.
-ALL_FORMATS = dict(FORMATS, ape=Format((24, 90), (16, 24), build_ape))
+# which tests/test_load_tool_ape.py and tests/test_load_tool_tak.py build in the same way.
+ALL_FORMATS = dict(FORMATS, ape=Format((24, 90), (16, 24), build_ape), tak=Format((24, 90), (16, 24), build_tak))
 
 
 def cases(name, minutes, bits):
