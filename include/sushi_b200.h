@@ -39,7 +39,7 @@
 extern "C" {
 #endif
 
-#define SB_ABI_VERSION 17
+#define SB_ABI_VERSION 18
 
 /* status codes */
 #define SB_OK            0
@@ -57,6 +57,7 @@ typedef struct sb_pcm sb_pcm;            /* opaque: decoded interleaved int16 PC
 typedef struct sb_ts sb_ts;              /* opaque: one audio PID of an MPEG transport stream being demuxed */
 typedef struct sb_ps sb_ps;              /* opaque: one audio stream of an MPEG program stream being demuxed */
 typedef struct sb_ogg sb_ogg;            /* opaque: one FLAC stream of an Ogg file being demuxed */
+typedef struct sb_avi sb_avi;            /* opaque: one audio stream of an AVI file being demuxed */
 
 /* ---- life cycle ------------------------------------------------------- */
 
@@ -446,6 +447,34 @@ int sb_ogg_open(uint32_t serial, int32_t channels, int32_t bits, int32_t rate, i
 int sb_ogg_feed(sb_ogg* ogg, const void* host_chunk, int64_t nbytes, int64_t file_offset);
 int sb_ogg_finish(sb_ogg* ogg, int32_t* cut, sb_pcm** out);
 int sb_ogg_destroy(sb_ogg* ogg);
+
+/* ---- AVI (ABI version 18) ----------------------------------------------------------------------------------------
+ *
+ * One audio stream of an AVI file (OpenDML included), demuxed on the GPU: the payloads of its `NNwb` chunks (NN the
+ * two decimal digits of stream_index, 0 to 99) in file order.  movi_extents[2 e], movi_extents[2 e + 1] are the file
+ * offsets of the first chunk and the end of movi list e (sorted, none empty): the `LIST movi` of `RIFF AVI ` and of
+ * each `RIFF AVIX`.  The file is fed in chunks of any size, in order; the host does no per-chunk work.  Chunks have
+ * variable sizes and may straddle feeds: every chunk header of a feed (`NNwb`, `NNdc`, `NNdb`, `NNpc`, `NNtx`,
+ * `ix##`, `JUNK`, `LIST rec `) is found, each links to the one its size (padded to even) reaches, `LIST rec ` to its
+ * first child and a list's last chunk to the next list's first, and the chain from the position the previous feed
+ * reached is found by pointer jumping; bytes the chain jumps over are not copied.  codec:
+ *   SB_AVI_PCM  config[0..2] = channels (1 to 8), bits (16 or 24), rate: little-endian interleaved PCM, stored as
+ *               sb_pcm_from_le stores it (24-bit samples by their top 16 bits); every chunk must hold whole sample
+ *               frames;
+ *   SB_AVI_MP2  the payloads are one MPEG audio stream, decoded as SB_TS_MP2 decodes a PID (config is not read);
+ *               messages about a frame name the file offset of the chunk holding its header.
+ * Damage fails with SB_EINVAL, "AVI chunk at byte offset N: ...", naming: a position the chain reaches that holds no
+ * chunk header (a broken FOURCC, a wrong size, bytes between chunks), a chunk whose size runs past its movi list, a
+ * PCM chunk that is not whole sample frames.  A last chunk cut by the file's end keeps the bytes there are and sets
+ * *cut, as does a chain that stops short of the last list's end.  sb_avi_feed returns once the chunk is copied and
+ * scanned for chunk headers.  The sb_pcm outlives the sb_avi. */
+#define SB_AVI_PCM 0
+#define SB_AVI_MP2 1
+int sb_avi_open(int32_t stream_index, int32_t codec, const int32_t* config, const int64_t* movi_extents,
+                int64_t n_extents, sb_avi** out);
+int sb_avi_feed(sb_avi* avi, const void* host_chunk, int64_t nbytes, int64_t file_offset);
+int sb_avi_finish(sb_avi* avi, int32_t* cut, sb_pcm** out);
+int sb_avi_destroy(sb_avi* avi);
 
 /* ---- multi-GPU: events shard across ranks (SURVEY.md 8e) ---------------- */
 

@@ -17,7 +17,7 @@ LIB_PATH = os.path.join(_HERE, 'libsushi_b200.so')
 
 SB_OK = 0
 SB_U8, SB_F32 = 0, 1
-ABI_VERSION = 17
+ABI_VERSION = 18
 SB_TS_PCM_BLURAY, SB_TS_TRUEHD, SB_TS_MP2 = 0, 1, 2
 
 c_i64 = ctypes.c_int64
@@ -101,6 +101,10 @@ PROTOTYPES = {
     'sb_ogg_feed': (ctypes.c_int, [c_vp, c_vp, c_i64, c_i64]),
     'sb_ogg_finish': (ctypes.c_int, [c_vp, c_i32p, ctypes.POINTER(c_vp)]),
     'sb_ogg_destroy': (ctypes.c_int, [c_vp]),
+    'sb_avi_open': (ctypes.c_int, [ctypes.c_int32, ctypes.c_int32, c_i32p, c_i64p, c_i64, ctypes.POINTER(c_vp)]),
+    'sb_avi_feed': (ctypes.c_int, [c_vp, c_vp, c_i64, c_i64]),
+    'sb_avi_finish': (ctypes.c_int, [c_vp, c_i32p, ctypes.POINTER(c_vp)]),
+    'sb_avi_destroy': (ctypes.c_int, [c_vp]),
     'sb_comm_unique_id': (ctypes.c_int, [c_vp]),
     'sb_comm_init': (ctypes.c_int, [c_vp, ctypes.c_int, ctypes.c_int]),
     'sb_comm_destroy': (ctypes.c_int, []),
@@ -190,8 +194,8 @@ def decode_frames(device, name, data, offsets, blocks, *args):
 
 
 def demux_file(device, prefix, open_args, path, chunk_bytes, align=1):
-    """The file at `path` demuxed and decoded on the GPU by a chunked demultiplexer (`prefix` 'sb_ts', 'sb_ps' or
-    'sb_ogg'):
+    """The file at `path` demuxed and decoded on the GPU by a chunked demultiplexer (`prefix` 'sb_ts', 'sb_ps',
+    'sb_ogg' or 'sb_avi'):
     <prefix>_open(*open_args), the file fed in chunks of chunk_bytes rounded down to whole `align`-byte packets,
     <prefix>_finish, and <prefix>_destroy however that ends.  Returns (sb_pcm handle, the cut flag finish set, the bytes
     of a partial last packet, which are not fed).  Every chunk goes through one page-locked buffer: a feed returns only

@@ -109,9 +109,9 @@ def create_arg_parser():
                         help='Timecodes file to use instead of making one from the source (when possible)')
 
     parser.add_argument('--src', required=True, dest='source', metavar='<filename>',
-                        help='Source audio or video (WAV, FLAC, WavPack, TTA, APE, TAK, TrueHD, Matroska, MP4, MPEG-TS or Ogg)')
+                        help='Source audio or video (WAV, FLAC, WavPack, TTA, APE, TAK, TrueHD, Matroska, MP4, MPEG-TS, Ogg or AVI)')
     parser.add_argument('--dst', required=True, dest='destination', metavar='<filename>',
-                        help='Destination audio or video (WAV, FLAC, WavPack, TTA, APE, TAK, TrueHD, Matroska, MP4, MPEG-TS or Ogg)')
+                        help='Destination audio or video (WAV, FLAC, WavPack, TTA, APE, TAK, TrueHD, Matroska, MP4, MPEG-TS, Ogg or AVI)')
     parser.add_argument('-o', '--output', default=None, dest='output_script', metavar='<filename>',
                         help='Output script')
 
@@ -122,7 +122,7 @@ def create_arg_parser():
 
 
 def _open_input(path):
-    """The opened reader of a container input (inputs.READERS: Matroska, MP4, Ogg, transport or program stream), which also
+    """The opened reader of a container input (inputs.READERS: Matroska, MP4, Ogg, AVI, transport or program stream), which also
     gives its script, chapters and streams; None for a WAV, FLAC, raw TrueHD (.thd), WavPack (.wv), TTA (.tta), Monkey's
     Audio (.ape), TAK (.tak) or MPEG audio (.mp2, .mpa, .m2a) input,
     which WavStream reads.  Any other extension, or a container's that does not open as one, is refused where the

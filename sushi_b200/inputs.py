@@ -3,7 +3,7 @@ them all) with one method, select_audio(track=None), which makes every refusal t
 common.Audio WavStream loads.  WavStream detects the format (open_input); the command line goes by file extension."""
 import collections
 
-from . import ape, matroska, mp4, mpa, mpegps, mpegts, ogg, tak, truehd, tta, wavpack
+from . import ape, avi, matroska, mp4, mpa, mpegps, mpegts, ogg, tak, truehd, tta, wavpack
 from .flac import FlacFile, is_flac
 from .wav import DownmixedWavFile
 
@@ -42,13 +42,18 @@ APE_FORMATS = (
 TAK_FORMATS = (
     Format('TAK', tak.TAK_EXTENSIONS, tak.is_tak, tak.TakFile, None),
 )
+# AVI files, known by `RIFF` + size + `AVI `, asked after those and before the table above (whose WAV reader takes every
+# other RIFF file)
+AVI_FORMATS = (
+    Format('AVI', avi.AVI_EXTENSIONS, avi.is_avi, avi.AviFile, 'an AVI file'),
+)
 # READERS is the whole table, in the order open_input asks.
-READERS = MPEG_FORMATS + OGG_FORMATS + APE_FORMATS + TAK_FORMATS + FORMATS
+READERS = MPEG_FORMATS + OGG_FORMATS + APE_FORMATS + TAK_FORMATS + AVI_FORMATS + FORMATS
 
 
 def open_input(source):
     """(reader, format name) of `source`: a file name, whose format is detected by content, or an opened container
-    reader (MatroskaFile, Mp4File, TransportStream, ProgramStream, OggFile), which is returned as it is and never
+    reader (MatroskaFile, Mp4File, TransportStream, ProgramStream, OggFile, AviFile), which is returned as it is and never
     sniffed."""
     for f in READERS:
         if f.opens_as and isinstance(source, f.reader):

@@ -29,7 +29,7 @@ import numpy as np  # noqa: E402
 
 from sushi_b200 import _native, matroska, mp4, mpegts, tta, wavpack  # noqa: E402
 from sushi_b200.wavstream import FlacFile, WavStream  # noqa: E402
-from tests import (alac_cases, ape_cases, flac_cases as fc, loader_cases as lc, mkv_cases, mp2_cases,  # noqa
+from tests import (alac_cases, ape_cases, avi_cases, flac_cases as fc, loader_cases as lc, mkv_cases, mp2_cases,  # noqa
                    mp4_cases, ogg_cases, ps_cases, ref_mp2, ref_swr, tak_cases, truehd_cases, ts_cases, tta_cases,
                    wavpack_cases)
 
@@ -363,6 +363,14 @@ def build_tak(directory, minutes, bits):
                  ('flac', flac), ('wav', wav))
 
 
+def build_avi(directory, minutes, bits):
+    """tests/avi_cases.py's long OpenDML file: 1 s chunks of 48 kHz stereo PCM beside 4 kB chunks of random-byte video,
+    RIFF AVI up to 1 GiB and RIFF AVIX lists after it."""
+    path = os.path.join(directory, 'avi%d_%d.avi' % (minutes, bits))
+    avi_cases.long_file(path, minutes, bits)
+    return sized({'minutes': minutes, 'bits': bits}, ('avi (PCM)', path))
+
+
 PS_PACK = 2048
 PS_VIDEO_PER_AUDIO = 11              # video packs between audio packs: about 1.5 GB for 90 minutes
 
@@ -539,8 +547,9 @@ FORMATS = {
 
 
 # Every format the tool measures: FORMATS, and the formats added after tests/test_load_tool.py's table of input kinds,
-# which tests/test_load_tool_ape.py and tests/test_load_tool_tak.py build in the same way.
-ALL_FORMATS = dict(FORMATS, ape=Format((24, 90), (16, 24), build_ape), tak=Format((24, 90), (16, 24), build_tak))
+# which tests/test_load_tool_ape.py, tests/test_load_tool_tak.py and tests/test_load_tool_avi.py build in the same way.
+ALL_FORMATS = dict(FORMATS, ape=Format((24, 90), (16, 24), build_ape), tak=Format((24, 90), (16, 24), build_tak),
+                   avi=Format((90,), (16, 24), build_avi))
 
 
 def cases(name, minutes, bits):
